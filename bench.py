@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- inner-loop solves/sec of the ICNN argmin path on B200 (BASELINE.json metric).
+"""bench.py -- inner-loop solves/sec of the ICNN argmin path on an H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C5] [--scaling strong|weak] [--impl reference]
+                    [--dump-outputs DIR]
 
 One "step" = one solveBatch over one minibatch of synthetic input.  Headline workload (default) = C5 =
 BASELINE.json configs[4], the largest single-GPU configuration (n_y=4096, 4x1024 hidden, batch 8192,
@@ -21,8 +22,11 @@ iterations-executed honours the reference's early return, lib/bundle_entropy.py:
                T (batch 4096 / n_y 512), C2 (Olivetti dims), C3 (Bibtex dims: bundle AND 30-step GD), C4 (RL dims),
                each with its own value / e2e / roofline / cpu_baseline
 
---impl reference: times the CPU implementation only (oracle port; the reference itself is Python and
-/root/reference does not exist on the GPU box), all host cores, same metric/config; loads no native code.
+--impl reference: times the CPU implementation only (oracle port; the reference itself is Python 2 / TensorFlow
+code that is not part of this repository), all host cores, same metric/config; loads no native code.
+
+--dump-outputs DIR: after the timed steps, the outputs of the headline workload's last step go to DIR/<name>.npy
+(dump_outputs).  The inputs are seeded, so two builds run with the same arguments can be compared file by file.
 """
 import argparse
 import json
@@ -51,18 +55,9 @@ def load_peaks():
         return dict(hbm_gbs=float(pk["hbm_gbs"]), bf16_tflops=float(pk["bf16_tflops"]),
                     bf16_sustained=float(pk.get("bf16_tflops_sustained", pk["bf16_tflops"])),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0,
-                source="fallback (B200_PROFILING.md)")
-
-
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` captures (profiles/r02_traffic.json: {workload: {kernel, t, bytes, source}})."""
-    path = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            return json.load(f)
-    return {}
+    # H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s -- not measured
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0,
+                source="H100 SXM data sheet (not measured)")
 
 
 def workload_string(name, cfg, solver="pc"):
@@ -292,6 +287,46 @@ class Ctx:
     pass
 
 
+DUMP_BYTES = 48 * 1024 * 1024     # per --dump-outputs directory (every file counted)
+
+
+def dump_outputs(st, out_dir, y_all=None):
+    """What solveBatch hands its caller after the last timed step -- x = y* [B, n] and, per sample, the active
+    bundle A (rows of G), b, lam, xs in the order of the ragged views (BundleState._fetch), plus nIters -- as
+    float64 / float32 .npy files.  Rows are a fixed seeded sample of the whole batch (every row when the budget
+    allows; rows.npy holds their indices); A/b/lam/xs are padded to KS slots with zeros past each sample's count
+    (count.npy).  With several GPUs (``y_all`` = the gathered y*, what the sharded API returns) the same rows as on
+    one GPU are dumped, but x only: the bundles stay on the rank that owns each row."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    B = st.B if y_all is None else y_all.shape[0]
+    n, KS = st.n, st.KS
+    per_row = n * 8 + KS * n * 4 + (KS * n * 8 if st.ys is not None else 0) + 2 * KS * 8 + 16
+    R = max(1, min(B, DUMP_BYTES // per_row))
+    rows = np.arange(B) if R == B else np.sort(np.random.RandomState(0).choice(B, R, replace=False))
+    ri = torch.as_tensor(rows, dtype=torch.int64, device=st.y.device)
+    if y_all is not None:
+        for k, v in (("rows", torch.as_tensor(rows, dtype=torch.float64)), ("x", y_all.index_select(0, ri))):
+            np.save(os.path.join(out_dir, k + ".npy"), v.cpu().numpy())
+        return
+    count = st.count.index_select(0, ri).to(torch.int64)
+    live = torch.arange(KS, device=st.y.device)[None, :] < count[:, None]
+    slot = torch.where(live, st.perm.index_select(0, ri).to(torch.int64), torch.zeros_like(count)[:, None])
+
+    def bundle(src):
+        v = src.index_select(0, ri)
+        v = v.gather(1, slot[..., None].expand(-1, -1, n)) if v.dim() == 3 else v.gather(1, slot)
+        return torch.where(live.view(live.shape + (1,) * (v.dim() - 2)), v, torch.zeros_like(v))
+
+    out = {"rows": torch.as_tensor(rows, dtype=torch.float64), "x": st.y.index_select(0, ri),
+           "A": bundle(st.G), "b": bundle(st.h), "lam": bundle(st.lam), "count": count.to(torch.float64),
+           "nIters": st.nIters.index_select(0, ri).to(torch.float64)}
+    if st.ys is not None:
+        out["xs"] = bundle(st.ys)
+    for k, v in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v.cpu().numpy())
+
+
 def measure_fp64_peak(ctx):
     """FP64 tensor-core (DMMA m8n8k4) throughput of this GPU, measured live: the denominator of K2's roofline
     (MEASURED_PEAKS.json carries HBM and bf16 only)."""
@@ -313,8 +348,9 @@ def measure_fp64_peak(ctx):
     return best
 
 
-def measure_workload(ctx, name, steps, warmup, scaling, solver, cpu_seconds, headline):
-    """value / e2e / per-kernel roofline / cpu_baseline of one workload on this rank set."""
+def measure_workload(ctx, name, steps, warmup, scaling, solver, cpu_seconds, headline, dump_dir=None):
+    """value / e2e / per-kernel roofline / cpu_baseline of one workload on this rank set; with ``dump_dir``, rank 0
+    writes the outputs of the last timed step there (``dump_outputs``)."""
     import ctypes as C
     import torch
     import torch.distributed as dist
@@ -402,6 +438,8 @@ def measure_workload(ctx, name, steps, warmup, scaling, solver, cpu_seconds, hea
         clk.__exit__()
     ms_per_step = allmax(sum(a.elapsed_time(b) for a, b in ev)) / steps
     value = Bglob * its / (ms_per_step * 1e-3)
+    if dump_dir and rank == 0:       # before the passes below reuse the state
+        dump_outputs(st, dump_dir, y_all if world > 1 else None)
 
     # ---- the same loop replayed from a CUDA graph (icnn_loop_graph_*): device time and HOST enqueue time of both
     # forms -- what "launch-bound or not" means for this workload (VERDICT r01 item 5)
@@ -519,17 +557,9 @@ def measure_workload(ctx, name, steps, warmup, scaling, solver, cpu_seconds, hea
     # K2: bound by the FP64 pipe (DMMA Gram + FP64 vector work); SURVEY.md 8d's HBM model kept beside it
     k2_flops = k2_fp64_flops(n, stats)
     k2_bytes = 4.0 * n * (ksum + 2.0 * B * its) + 8.0 * ksum
-    tr = ctx.traffic.get(name, {})
-
-    def _traffic(kname):
-        t_ = tr.get(kname)
-        if not t_:
-            return None, None
-        return t_["bytes"] * (float(B) / t_["rows"]), "%s; %d rows captured, scaled to %d rows (independent samples)" % (t_["source"], t_["rows"], B)
     roof_k2 = dict(kernel=k2_name, bound="tensor", pipe="fp64 tensor core (DMMA m8n8k4) + FP64 FMA",
                    achieved=k2_flops / (k2_ms * 1e-3) / 1e12, peak=ctx.fp64_peak, unit="TFLOP/s",
                    peak_source="measured live (icnn_fp64_mma_probe, DMMA)",
-                   traffic=_traffic("K2")[0], traffic_source=_traffic("K2")[1],
                    launches=its, ms_per_launch=k2_ms / max(its, 1), share_of_step=k2_ms / (k1_ms + k2_ms),
                    ms_per_launch_with_statistics=k2_ms_stats / max(its, 1),
                    algorithmic_gflop_per_step=k2_flops / 1e9,
@@ -541,12 +571,11 @@ def measure_workload(ctx, name, steps, warmup, scaling, solver, cpu_seconds, hea
                                        "its rows from L2 2-5 times per interior-point iteration and is FP64-bound"))
     roof_k2["frac"] = roof_k2["achieved"] / roof_k2["peak"] if roof_k2["peak"] else None
     k1_flops = flop_fg(cfg) * B * its
-    k1_name = ("tc_gemm_kernel (tcgen05 3xTF32 + TMA) + gate_y + out_layer" if tc_on
+    k1_name = ("tc_gemm_kernel (wgmma 3xTF32 + TMA) + gate_y + out_layer" if tc_on
                else "gated_gemm_kernel + out_layer (FP32 FFMA)")
     nl_k1 = its * (2 * L + 2)
     roof_k1 = dict(kernel=k1_name, bound="tensor", achieved=k1_flops / (k1_ms * 1e-3) / 1e12,
                    peak=peaks["bf16_sustained"], unit="TFLOP/s", peak_source=peaks["source"] + ", bf16 sustained",
-                   traffic=_traffic("K1")[0], traffic_source=_traffic("K1")[1],
                    launches=nl_k1, ms_per_launch=k1_ms / max(nl_k1, 1), share_of_step=k1_ms / (k1_ms + k2_ms),
                    note="FP32-accurate GEMMs as 3 TF32 MMAs per product: the ceiling of this formulation is "
                         "tf32 peak / 3 = bf16 peak / 6",
@@ -644,14 +673,14 @@ def run_gpu(args):
     ctx.dev = torch.device("cuda", ctx.local)
     if ctx.world > 1:
         dist.init_process_group("nccl", device_id=ctx.dev)
-    ctx.flush = torch.empty(512 * 1024 * 1024, dtype=torch.uint8, device=ctx.dev)   # > 126 MB L2
+    ctx.flush = torch.empty(512 * 1024 * 1024, dtype=torch.uint8, device=ctx.dev)   # > 50 MB L2
     ctx.stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     ctx.peaks = load_peaks()
-    ctx.traffic = load_traffic()
     ctx.fp64_peak = measure_fp64_peak(ctx)
     scaling = args.scaling or "strong"
     cpu_s = 0.0 if args.no_cpu_baseline else args.cpu_seconds
-    head = measure_workload(ctx, args.workload, args.steps, max(3, args.warmup), scaling, args.solver, cpu_s, True)
+    head = measure_workload(ctx, args.workload, args.steps, max(3, args.warmup), scaling, args.solver, cpu_s, True,
+                            dump_dir=args.dump_outputs)
     subs = {}
     if ctx.world == 1 and not args.no_sub:
         for w in SUB_WORKLOADS:
@@ -744,7 +773,11 @@ def main():
     ap.add_argument("--cpu-seconds", type=float, default=15.0)
     ap.add_argument("--sub-cpu-seconds", type=float, default=6.0)
     ap.add_argument("--sub-steps", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the headline workload's last timed step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.no_sub = args.no_sub or args.no_target_shape
     try:
         if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""icnn_b200 -- B200-native inner loop argmin_y f(x, y; theta) of locuslab/icnn.
+"""icnn_b200 -- H100-native inner loop argmin_y f(x, y; theta) of locuslab/icnn.
 
 Public surface (mirrors the reference's, see INTEGRATION.md):
     icnn_b200.bundle_entropy.solveBatch(fg, initXs, nIter, callback, solver, variant=...)
@@ -6,7 +6,7 @@ Public surface (mirrors the reference's, see INTEGRATION.md):
     icnn_b200.gd.solve(...)              -> unrolled momentum gradient descent
     icnn_b200.argmin_grad.argmin_grad(state, trueY, loss) -> crossEntrGrad / mseGrad + train_step_fd feeds
     icnn_b200.gd_grad.gd_grad(fg, y0, trueY, ...) -> d mse / d theta through the unrolled GD loop
-The compute path is hand-written sm_100a CUDA behind a C ABI (libicnn_b200.so).  Every attribute above
+The compute path is hand-written sm_90a CUDA behind a C ABI (libicnn_b200.so).  Every attribute above
 loads the native library on first use and raises ImportError when it is missing -- there is no CPU
 fallback.  Only ``icnn_b200.workloads`` (pure-numpy synthetic inputs, shared with the CPU reference arm of
 bench.py) imports without it, so that the reference arm maps no native code.

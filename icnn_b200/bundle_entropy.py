@@ -1,6 +1,6 @@
-"""Drop-in ``solveBatch`` of the reference's bundle-entropy library, running on a B200.
+"""Drop-in ``solveBatch`` of the reference's bundle-entropy library, running on an H100.
 
-Reference surfaces reproduced (paths under /root/reference):
+Reference surfaces reproduced (paths relative to the locuslab/icnn repository):
     lib/bundle_entropy.py:192        solveBatch(fg, initXs, nIter=10, callback=None, solver='pc')
     lib/bundle_entropy_dual.py:129   solveBatch(fg, initXs, nIter=10, callback=None)
     RL/src/bundle_entropy.py:85      solveBatch(fg, initXs, nIter=5,  callback=None)
@@ -94,7 +94,7 @@ class BundleState:
         self.f64 = e(B, dtype=f64) if keep_f64 else None
         self.iter_stats = torch.zeros(nIter, _capi.NSTAT, dtype=torch.float64, device=device) if stats else None
         # scratch for the measured-and-rejected variant of the predictor-corrector kernel that keeps the per-sample
-        # n-vectors in L2 instead of shared memory (include/icnn_b200.h: vec_ws; profiles/r02_k2_sweep.md): only
+        # n-vectors in L2 instead of shared memory (include/icnn_b200.h: vec_ws): only
         # allocated when the exploration knob ICNN_PC_GV is set
         import os
         self.vec_ws = e(B, 4, (n + 15) & ~15, dtype=f64) if os.environ.get("ICNN_PC_GV") else None

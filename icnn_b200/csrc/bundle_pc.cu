@@ -51,11 +51,7 @@ static bool pc_fits(const icnn_bundle_bufs* b, int wps, int nch, PcConfig* out, 
 static bool pick_pc(const icnn_bundle_bufs* b, PcConfig* out) {
   const int n = b->n;
   if (b->KS > 62) return false;   // k + 2 sweep rows in <= 8 row blocks
-  // measured on B200, K2 ms per solveBatch (profiles/r02_k2_sweep.md):
-  //   n = 159  (C3)            two-sweep WPS 1: 4.5 (128-register build; 5.2 at 80 registers), WPS 2: 6.4; five-sweep 6.9
-  //   n = 512  (T)             two-sweep WPS 1: 10.6, 2: 9.9, 4: 11.0;                                   five-sweep 9.4
-  //   n = 2048 (C2)            two-sweep WPS 8: 20.3 (18.3 with the k <= 32 stage), 16: 27.7;            five-sweep 19.4
-  //   n = 4096 (C5, 1024 rows) two-sweep WPS 16: 203;                                                    five-sweep 224
+  // Chosen by K2 time per solveBatch, measured per shape on an earlier GPU (not re-measured on H100):
   // -> the two-sweep kernel where it wins (small and very large n_y), the five-sweep kernel in between.
   int wps, nch;
   if (n <= 128) { wps = 1; nch = 1; }
@@ -85,8 +81,8 @@ static bool pick_pc(const icnn_bundle_bufs* b, PcConfig* out) {
       if (force && n > 1024 && n <= 2048 && pc_fits(b, 4, 4, out, false, true)) return true;
     }
   }
-  // 256 < n_y <= 1024 stays on the five-sweep kernel (T: 9.34 vs 9.18 ms, inside the run-to-run spread); with the lean
-  // k <= 32 stage the two-sweep kernel wins at n_y = 2048 (C2: 18.3 vs 19.4 ms; ICNN_PC_5SWEEP=1 restores the old choice)
+  // 256 < n_y <= 1024 stays on the five-sweep kernel (a tie within the run-to-run spread); with the lean k <= 32 stage
+  // the two-sweep kernel won at n_y = 2048 (ICNN_PC_5SWEEP=1 restores the old choice)
   if (n > 256 && n <= 1024 && !getenv("ICNN_PC_WPS")) return false;
   if (n > 1024 && n <= 2048 && getenv("ICNN_PC_5SWEEP") && !getenv("ICNN_PC_WPS")) return false;
   if (const char* v = getenv("ICNN_PC_WPS")) {

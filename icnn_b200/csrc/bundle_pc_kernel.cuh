@@ -1,7 +1,7 @@
 // K2, Mehrotra predictor-corrector path (solver = ICNN_SOLVER_PC): two sweeps over the bundle rows per
 // interior-point iteration instead of five.
 //
-// Same algorithm, start and stopping rule as the reference's pdipm_pc (/root/reference/lib/bundle_entropy.py:5-78)
+// Same algorithm, start and stopping rule as the reference's pdipm_pc (lib/bundle_entropy.py:5-78)
 // and the same per-sample loop body as bundle_step_kernel (append, dependency test, prune:
 // lib/bundle_entropy.py:211-237); what changes is how the O(k n) work of one iteration is organised:
 //

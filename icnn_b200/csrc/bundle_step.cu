@@ -75,10 +75,10 @@ static int pick_k2(const icnn_bundle_bufs* b, K2Config* out) {
   }
   int want_cs = 0;
   if (const char* v = getenv("ICNN_K2_CS")) want_cs = atoi(v);
-  // Resident rows / cluster split are OFF by default: measured on B200 (round 1) they lose to
-  // streaming the rows from L2 on every configuration (C2 53.7 vs 20.4 ms, T 17.7 vs 9.4 ms,
-  // C5/512 773 vs 188 ms per solveBatch) -- the per-sample solve is a latency-bound FP64 chain, and
-  // what hides it is the number of samples in flight per SM, which residency divides by 3-5.
+  // Resident rows / cluster split are OFF by default: they lost to streaming the rows from L2 on every
+  // configuration when measured on an earlier GPU (not re-measured on H100) -- the per-sample solve is a
+  // latency-bound FP64 chain, and what hides it is the number of samples in flight per SM, which
+  // residency divides by 3-5.
   const char* rv = getenv("ICNN_K2_RESIDENT");
   const bool allow_res = (rv && rv[0] == '1');
   const size_t big = 200 * 1024, half = 110 * 1024;

@@ -1,7 +1,7 @@
 // K2: one outer iteration of the bundle-entropy method for every unfinished sample.
 //
 // Restates on the GPU the per-sample loop body of the reference's three solveBatch copies
-// (paths under /root/reference):
+// (paths relative to the locuslab/icnn repository):
 //   lib/bundle_entropy.py:211-237        append row, SVD rank stop, pdipm_pc (:5-78), prune lam<=1e-8
 //   lib/bundle_entropy_dual.py:148-174   append, rank stop, proj_newton_logistic (:15-85), prune lam<=0
 //   RL/src/bundle_entropy.py:106-131     append, Newton (:14-83), clip [.03,.97], |dy|<1e-6 stop

@@ -1,4 +1,4 @@
-// Shared helpers for libicnn_b200.so (sm_100a only).
+// Shared helpers for libicnn_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -32,6 +32,13 @@ void set_error(const char* fmt, ...);
   } while (0)
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+// streaming multiprocessors of the current device (132 on an H100 SXM): the grid-size heuristics aim at it
+static inline int device_sms() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 132;
+  return sms;
+}
 #ifdef __CUDACC__
 // optional per-outer-iteration statistics (icnn_bundle_bufs::iter_stats), totals over samples
 __device__ __forceinline__ void stat_add(double* st, int t, int idx, double v) {

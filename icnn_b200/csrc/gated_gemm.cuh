@@ -208,7 +208,8 @@ static cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st) {
   const int gx = cdiv(a.N, BN), gy = cdiv(a.M, BM);
   const int nk = cdiv(a.K0 + a.K1, BK);
   int S = 1;
-  while (S < 8 && gx * gy * S < 296 && nk / (S * 2) >= 4) S *= 2;
+  const int target = 2 * device_sms();
+  while (S < 8 && gx * gy * S < target && nk / (S * 2) >= 4) S *= 2;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(gx, gy, S);
   cfg.blockDim = dim3(256);

@@ -20,7 +20,7 @@
 // GDB epilogues of tc_gemm_kernel keep Z_l^(i), delta_l^(i) and delta_l^(i) Wz_l^T of every iteration
 // in HBM and accumulate Delta_l (kappa does not depend on a).  With a known, Ty_l = (a o cy_l) Wy_l is
 // iteration-independent, zt_0^(i) = act'(Z_0^(i)) o Ty_0 is elementwise, and per hidden layer ONE
-// tcgen05 GEMM over all iterations (M = nIter*B) gives zt_l, ONE weight-gradient GEMM (K = nIter*B)
+// wgmma GEMM over all iterations (M = nIter*B) gives zt_l, ONE weight-gradient GEMM (K = nIter*B)
 // gives dWz_l, and tangent_stage_kernel reduces dcz_l over the iterations.
 // Two-pass mode (fallback; also the FP32 FFMA path for B < 64): pass 1 -> y_N, pass 2 replays the
 // deterministic loop (bit-identical iterates) with, per iteration, the tangent forward (the same
@@ -160,7 +160,8 @@ static cudaError_t launch_wgrad(const WgradArgs& a, cudaStream_t st) {
   const int gx = cdiv(a.N, BN), gy = cdiv(a.M, BM);
   const int nk = cdiv(a.Kb, BK);
   int S = 1;
-  while (S < 8 && gx * gy * S < 296 && nk / (S * 2) >= 4) S *= 2;
+  const int target = 2 * device_sms();
+  while (S < 8 && gx * gy * S < target && nk / (S * 2) >= 4) S *= 2;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(gx, gy, S);
   cfg.blockDim = dim3(256);

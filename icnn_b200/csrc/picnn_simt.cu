@@ -11,7 +11,7 @@
 // backward: the same buffer read transposed), with the per-sample gates applied while the A tile
 // is staged and bias/activation/act'-mask/g-accumulate fused into the epilogue.  The width-1
 // output layer and its backward seed are a warp-per-sample kernel (shuffle reduction).
-// This FP32 kernel is the accuracy anchor for the tcgen05 path (picnn_tc.cu).
+// This FP32 kernel is the accuracy anchor for the wgmma path (picnn_tc.cu).
 #include "gated_gemm.cuh"
 
 #include <cstdlib>
@@ -167,7 +167,7 @@ int picnn_fg_simt(const icnn_picnn* h, const icnn_gates* gt, const float* y32, f
   return ICNN_OK;
 }
 
-// K1 dispatch: tcgen05 path once there are enough rows to fill a 128-row tile, FP32 FFMA path
+// K1 dispatch: wgmma path once there are enough rows to fill a 128-row tile, FP32 FFMA path
 // otherwise.  ICNN_K1=simt at handle creation keeps everything on the FFMA path.
 int picnn_fg_dispatch(const icnn_picnn* h, const icnn_gates* gt, const float* y32, float* f, float* g,
                       long long g_row_stride, const int* perm, const int* count, int KS, void* workspace,

@@ -1,23 +1,23 @@
-// K1 (tensor-core path): PICNN f and df/dy with tcgen05.mma (kind::tf32, 3xTF32 split for
-// FP32-level accuracy), operands staged by TMA into 128B-swizzled shared memory, accumulators in
-// TMEM, fused epilogues read back with tcgen05.ld.
+// K1 (tensor-core path): PICNN f and df/dy with Hopper warpgroup MMA (wgmma.mma_async, tf32 inputs,
+// 3xTF32 split for FP32-level accuracy), operands staged by TMA into 128B-swizzled shared memory,
+// accumulators in registers, fused epilogues.
 //
 // Same math as picnn_simt.cu (multi-label-cls/icnn_ebundle.py:349-387,146; RL/src/icnn.py:356-404):
 //   forward  layer i : Z_i   = act( A'_i  Wcat_i + d_i ),   A'_i = [Z_{i-1} o cz_i | (s y + t) o cy_i]
 //   backward layer i : [delta_{i-1} | g +=] = delta_i Wcat_i^T  with the gate / act' epilogues
 // Every GEMM is  C[M,N] = A[M,K] * B[N,K]^T  with BOTH operands K-major (the library keeps the
-// weights in both orientations), each operand pre-split into hi = tf32(x) and lo = x - hi:
-//   C = A_hi B_hi + A_hi B_lo + A_lo B_hi     (three tcgen05.mma per k-step, one FP32 TMEM accumulator)
+// weights in both orientations; wgmma takes tf32 operands K-major only), each operand pre-split into
+// hi = tf32(x) and lo = x - hi:
+//   C = A_hi B_hi + A_hi B_lo + A_lo B_hi     (three wgmma per k-step into one FP32 accumulator)
 // Plain TF32 (10-bit mantissa) moves y* by 1e-3..1e-2 (SURVEY.md section 7, hard part 2); the split
 // restores ~2^-21 relative error.
 //
-// Kernel anatomy (192 threads, one 128 x BN output tile per CTA):
-//   warp 0      TMA producer   : cp.async.bulk.tensor.2d of A_hi/A_lo/B_hi/B_lo boxes (32 fp32 = 128 B
-//                                wide) into a NST-stage ring, mbarrier expect_tx
-//   warp 1      MMA issuer     : one elected lane issues 12 tcgen05.mma per stage, tcgen05.commit
-//                                releases the stage / signals the epilogue; also owns TMEM alloc
-//   warps 2..5  epilogue       : tcgen05.ld (32 lanes x 16 columns), fused bias/activation/gates,
-//                                global stores (each warp owns TMEM lanes 32*(warp%4)..+31)
+// Kernel anatomy (288 threads, one 128 x BN output tile per CTA):
+//   warps 0..7  two consumer warpgroups; warpgroup g owns tile rows 64g..64g+63.  Per 32-wide k-block
+//               it issues 12 wgmma m64nBNk8 (4 k-steps x {hi*hi, hi*lo, lo*hi}) and releases the stage;
+//               afterwards every warp runs the fused epilogue on the 16 rows its accumulators hold
+//   warp 8      TMA producer: cp.async.bulk.tensor.2d of A_hi/A_lo/B_hi/B_lo boxes (32 fp32 = 128 B
+//               wide) into an NST-stage ring, mbarrier expect_tx
 #include "common.cuh"
 
 #include <cuda.h>
@@ -63,8 +63,8 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, ui
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 // one lane of a converged warp, chosen by the hardware (elect.sync): unlike `lane == 0`, ptxas knows that exactly one
-// thread runs the guarded region, so single-thread instructions (tcgen05.mma / commit, cp.async.bulk.tensor) are
-// emitted straight instead of inside an ELECT / BRA.U.ANY loop over the active lanes
+// thread runs the guarded region, so the single-thread TMA issue is emitted straight instead of inside a loop over
+// the active lanes
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred = 0;
   asm volatile(
@@ -77,64 +77,65 @@ __device__ __forceinline__ bool elect_one_sync() {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// the 256 threads of the two consumer warpgroups (named barrier 1; the producer warp never joins it)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across the asynchronous MMA
+template <int R>
+__device__ __forceinline__ void fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int j = 0; j < R; ++j) asm volatile("" : "+f"(d[j])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, FP32 accumulator in registers of the
+// issuing warpgroup; scale_d = 0 overwrites D.  Fragment of thread (warp w of the warpgroup, lane l):
+//   d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c]
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+      "}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
 }
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+      "}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
 }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 128 B, 8-row atoms
-// of 1024 B (cute/arch/mma_sm100_desc.hpp SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64)).
+// shared-memory matrix descriptor (sm_90 wgmma), K-major operand, 128-byte swizzle, rows of 128 B,
+// 8-row atoms of 1024 B: start>>4 [0,14), LBO>>4 [16,30) (unused: the K extent of a stage is one
+// swizzle span), SBO>>4 [32,46) = 1024 B between 8-row atoms, layout SWIZZLE_128B = 1 at [62,64).
+// Every operand buffer starts on a 1024-byte boundary, so the base-offset field stays 0.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)0 << 16;                       // LBO: unused for a single 128B swizzle atom along K
-  d |= (uint64_t)((1024 >> 4) & 0x3FFF) << 32;  // SBO: 8 rows x 128 B between row atoms
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((1024 >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// instruction descriptor, kind::tf32: C=F32 (bit 4), A=B=TF32 (2 at bits 7, 10), K-major both,
-// N>>3 at [17,23), M>>4 at [24,29)  (cute/arch/mma_sm100_desc.hpp InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // TF32 split with round-to-nearest on both parts: hi = rn_tf32(x), lo = rn_tf32(x - hi), both exactly
@@ -149,13 +150,16 @@ __device__ __forceinline__ float tf32_lo(float x, float hi) { return tf32_rn(x -
 // ---------------------------------------------------------------------------------------------
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 32;  // fp32 elements per stage row = one 128-byte swizzle span
-constexpr int TC_CH = 1;   // default k-blocks per accumulation chunk (K = 32: four accumulations per TMEM accumulator before the RN
-                           // drain); TcArgs::ch carries the value a launch uses (ICNN_TC_CH, read once: accuracy/speed exploration)
-constexpr int TC_SETS = 3; // hi*hi accumulators in flight (+ one cross-term accumulator = 4 x BN TMEM columns)
+constexpr int TC_HALF = TC_BK / 16;   // k-steps (K = 8 each) per half k-block
+constexpr int TC_CH = 1;   // default half k-blocks per accumulation chunk (K = 16: 6 MMAs into the chunk accumulator before
+                           // the RN add into the running sum); TcArgs::ch carries the value a launch uses (ICNN_TC_CH,
+                           // read once: accuracy/speed exploration)
+constexpr int TC_CONSUMER_WARPS = 8;
+constexpr int TC_THREADS = 32 * (TC_CONSUMER_WARPS + 1);
 
 struct TcArgs {
   int M, N, K;
-  int ch;    // k-blocks per accumulation chunk (>= 1), set by launch_tc_gemm
+  int ch;    // half k-blocks per accumulation chunk (>= 1), set by launch_tc_gemm
   int mode;  // 0 forward, 1 backward, 2 plain store (self test)
   // forward epilogue: Z = act(acc + D); optional next-layer operand A'_{next}[:, 0:N] = Z o Cz_next (hi/lo)
   const float* D; float* Z; float alpha;
@@ -187,62 +191,45 @@ struct TcSmem {
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr int BAR_OFF = NST * STAGE_BYTES;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;  // + alignment slack
+  // the finished [TC_BM][BN + 1] tile is staged for the epilogue in the idle ring
+  static_assert(TC_BM * (BN + 1) * 4 <= BAR_OFF, "epilogue tile does not fit the ring");
 };
 
-// <128,3>: one CTA / SM (198 KB);  <64,4>: one CTA / SM, deeper ring for small grids;
-// <64,2>: two CTAs / SM (98 KB each, 2 x 256 TMEM columns) so that one CTA's epilogue overlaps
-// the other's main loop.
+// <128,3>: one CTA / SM (194 KB);  <64,4>: one CTA / SM, deeper ring for small grids;
+// <64,2>: two CTAs / SM (98 KB each) so that one CTA's epilogue overlaps the other's main loop.
 template <int BN, int NST_, bool GDB = false>
-__global__ void __launch_bounds__(192, (BN == 64 && NST_ == 2) ? 2 : 1)
+__global__ void __launch_bounds__(TC_THREADS, (BN == 64 && NST_ == 2) ? 2 : 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, TcArgs a) {
   if (a.skip_if_zero != nullptr && *a.skip_if_zero == 0) return;
   using SM = TcSmem<BN, NST_>;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment (128B swizzle atoms) as an OFFSET into the shared array: a pointer rebuilt from an integer
-  // (uintptr_t round-up) loses its address space, the read of the TMEM base address below becomes a GENERIC load,
-  // which the compiler must treat as lane-divergent -- and every tcgen05.mma then gets an ELECT / R2UR.BROADCAST /
-  // BRA.U.ANY "waterfall" around it (13 SASS instructions per MMA; ncu, round 2: the single MMA-issuing thread never
-  // waited on a barrier and the tensor pipe sat at 23-28 %: the kernel was bound by that thread's instruction stream).
+  // 1024-byte alignment (128B swizzle atoms) as an OFFSET into the shared array, so that every address below keeps
+  // the shared address space
   const uint32_t smem_pad = ((smem_u32(smem_raw) + 1023u) & ~1023u) - smem_u32(smem_raw);
   uint8_t* smem = smem_raw + smem_pad;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::BAR_OFF);
   uint64_t* empty = full + SM::NST;
-  uint64_t* acc_full = empty + SM::NST;           // [TC_SETS] hi*hi accumulator s holds a finished chunk
-  uint64_t* acc_empty = acc_full + TC_SETS;       // [TC_SETS] accumulator s has been drained by the four epilogue warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + TC_SETS);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
   // split-K: gridDim.z = S CTAs of one cluster share the output tile, each reduces a K-slice into its
-  // own TMEM accumulators; the partial tiles are summed through distributed shared memory below
+  // own accumulators; the partial tiles are summed through distributed shared memory below
   const int S = gridDim.z;
   const int nkb_all = (a.K + TC_BK - 1) / TC_BK;
   const int kb0 = (int)(((long long)nkb_all * blockIdx.z) / S);
   const int nkb = (int)(((long long)nkb_all * (blockIdx.z + 1)) / S) - kb0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmBh); tma_prefetch_desc(&tmBl);
-    for (int s = 0; s < SM::NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < TC_SETS; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+    // a stage is free again once each of the eight consumer warps has seen its MMAs complete
+    for (int s = 0; s < SM::NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  // Chunked accumulation (round 2).  The tensor core truncates its FP32 accumulator toward zero at every MMA:
-  // a systematic relative bias of ~3e-8 per accumulation (tools/tc_bias_probe.py: -1.2e-5 at K = 5120 in one
-  // accumulator chain, -1.2e-6 with K cut into 640-slices, -1.7e-7 with 128-slices), which compounds through
-  // the layers (C5: f scaled by 1 - 1.1e-5) and moves y* by 3e-3 over 50 bundle iterations.  The reduction is
-  // therefore cut into CHUNKS of TC_CH k-blocks: the MMA warp accumulates the hi*hi products of one chunk in TMEM
-  // accumulator (c % 3) while the four epilogue warps drain the finished ones into FP32 REGISTERS with
-  // round-to-nearest adds.  The 2^-11 smaller cross terms keep ONE accumulator for the whole reduction (their
-  // truncation bias is 2^-11 of 4e-5: nothing) and are added once at the end: the drain reads half the TMEM
-  // bytes and three hi*hi accumulators decouple the MMA issue from the drain.  4 x BN TMEM columns as before.
-  if (warp == 1) tmem_alloc(tmem_slot, 4 * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == TC_CONSUMER_WARPS) {
+    // ---- producer ----
     if (elect_one_sync()) {
       for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb % SM::NST;
@@ -258,271 +245,259 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      constexpr uint32_t idesc = make_idesc_tf32(TC_BM, BN);
-      const int CH = a.ch;
-      const int nch = (nkb + CH - 1) / CH;
-      const uint32_t xx = tmem_base + (uint32_t)(TC_SETS * BN);
-      for (int c = 0; c < nch; ++c) {
-        const int set = c % TC_SETS;
-        if (c >= TC_SETS) { mbar_wait(&acc_empty[set], (uint32_t)(((c / TC_SETS) - 1) & 1)); tc_fence_after(); }
-        const uint32_t hh = tmem_base + (uint32_t)(set * BN);
-        const int kb1 = ::min(nkb, (c + 1) * CH);
-        for (int kb = c * CH; kb < kb1; ++kb) {
-          const int s = kb % SM::NST;
-          const uint32_t ph = (kb / SM::NST) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t st = smem_u32(smem + s * SM::STAGE_BYTES);
-          const uint64_t dAh = make_kmajor_sw128_desc(st);
-          const uint64_t dAl = make_kmajor_sw128_desc(st + SM::A_BYTES);
-          const uint64_t dBh = make_kmajor_sw128_desc(st + 2 * SM::A_BYTES);
-          const uint64_t dBl = make_kmajor_sw128_desc(st + 2 * SM::A_BYTES + SM::B_BYTES);
+    // every thread of the cluster takes part in both cluster barriers of the split-K epilogue
+    if (S > 1) { cg::this_cluster().sync(); cg::this_cluster().sync(); }
+    return;
+  }
+
+  // ---- consumers: main loop ----
+  // Chunked accumulation.  The tensor core does not round its FP32 accumulator to nearest at every MMA, which
+  // leaves a systematic relative bias per accumulation (tools/tc_bias_probe.py) that compounds through the layers
+  // and moves y* over 50 bundle iterations.  The reduction is therefore cut into CHUNKS of a.ch half k-blocks: the
+  // products of one chunk (hi*hi and the 2^-11 smaller cross terms) go into the wgmma accumulator `frag`, which
+  // is then added into the FP32 running sum `run` with round-to-nearest adds.
+  // Each half-block waits for its own MMAs (wait_group 0) before the next is issued: the tensor core of an SM is
+  // kept busy by the other warpgroup and the second CTA, not by a deeper MMA pipeline within one warpgroup.
+  const int wg = warp >> 2;   // consumer warpgroup: tile rows 64 wg .. 64 wg + 63
+  float run[BN / 2], frag[BN / 2];
 #pragma unroll
-          for (int k4 = 0; k4 < TC_BK / 8; ++k4) {
-            const uint64_t adv = (uint64_t)((k4 * 8 * 4) >> 4);  // +32 B per k-step inside the swizzle span
-            const uint32_t first = (kb == c * CH && k4 == 0) ? 0u : 1u;
-            umma_tf32(hh, dAh + adv, dBh + adv, idesc, first);
-            umma_tf32(xx, dAh + adv, dBl + adv, idesc, (kb == 0 && k4 == 0) ? 0u : 1u);
-            umma_tf32(xx, dAl + adv, dBh + adv, idesc, 1u);
+  for (int j = 0; j < BN / 2; ++j) { run[j] = 0.f; frag[j] = 0.f; }
+  {
+    const int CH = a.ch;
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int s = kb % SM::NST;
+      const uint32_t ph = (kb / SM::NST) & 1;
+      mbar_wait(&full[s], ph);
+      const uint32_t st = smem_u32(smem + s * SM::STAGE_BYTES);
+      const uint32_t arow = (uint32_t)(wg * (SM::A_BYTES / 2));   // 64 rows x 128 B
+      const uint64_t dAh = make_kmajor_sw128_desc(st + arow);
+      const uint64_t dAl = make_kmajor_sw128_desc(st + SM::A_BYTES + arow);
+      const uint64_t dBh = make_kmajor_sw128_desc(st + 2 * SM::A_BYTES);
+      const uint64_t dBl = make_kmajor_sw128_desc(st + 2 * SM::A_BYTES + SM::B_BYTES);
+      // two half-blocks of K = 16 (TC_HALF k-steps each); chunk c covers half-blocks c*CH .. c*CH + CH - 1
+#pragma unroll
+      for (int hb = 0; hb < 2; ++hb) {
+        const int h = 2 * kb + hb;
+        const int first = (h % CH) == 0;
+        fence_operands(frag);
+        wgmma_fence();
+        // the 2^-11 smaller cross terms first, then the hi*hi products: an accumulation truncates at the
+        // accumulator's magnitude, so only the hi*hi steps add a truncation at full size
+#pragma unroll
+        for (int k = 0; k < TC_HALF; ++k) {
+          const uint64_t adv = (uint64_t)(((hb * TC_HALF + k) * 8 * 4) >> 4);  // +32 B per k-step inside the swizzle span
+          wgmma_tf32(frag, dAh + adv, dBl + adv, (first && k == 0) ? 0 : 1);
+          wgmma_tf32(frag, dAl + adv, dBh + adv, 1);
+        }
+#pragma unroll
+        for (int k = 0; k < TC_HALF; ++k) {
+          const uint64_t adv = (uint64_t)(((hb * TC_HALF + k) * 8 * 4) >> 4);
+          wgmma_tf32(frag, dAh + adv, dBh + adv, 1);
+        }
+        wgmma_commit();
+        wgmma_wait0();
+        fence_operands(frag);
+        if ((h + 1) % CH == 0 || h + 1 == 2 * nkb) {
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) run[j] += frag[j];
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);   // this warp's share of the stage has been read
+    }
+  }
+
+  // ---- epilogue: registers -> [TC_BM][BN + 1] tile in the idle ring -> fused epilogue -> global ----
+  // Warp w holds tile rows 16w..16w+15 (warpgroup w/4, warp w%4 of it).  Global traffic wants one row per
+  // warp instruction (lanes = consecutive columns), so the accumulators go through shared memory first.
+  consumer_sync();   // both warpgroups are done reading the ring
+  float* P = reinterpret_cast<float*>(smem);
+  constexpr int PP = BN + 1;
+  {
+    const int rb = warp * 16 + (lane >> 2), cb = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) P[(rb + 8 * i) * PP + 8 * j + cb + c] = run[4 * j + 2 * i + c];
+  }
+  if (S > 1) {
+    // ---- split-K epilogue: DSMEM sum of the cluster's partial tiles -> fused epilogue ----
+    // (every CTA of the cluster reaches both cluster barriers: the producer warp calls them above)
+    cg::this_cluster().sync();
+    cg::cluster_group cl = cg::this_cluster();
+    const int rank = (int)cl.block_rank();
+    const int rlo = (TC_BM * rank) / S, rhi = (TC_BM * (rank + 1)) / S;
+    for (int rr = rlo + warp; rr < rhi; rr += TC_CONSUMER_WARPS) {   // this warp's rows of the CTA's row slice
+      const int m = m0 + rr;
+      if (m >= a.M) break;
+      float* grow = nullptr;
+      if (a.mode == 1)
+        grow = (a.perm == nullptr) ? a.g + (long long)m * a.g_row_stride
+                                   : a.g + ((long long)m * a.KS + a.perm[(long long)m * a.KS + a.count[m]]) * a.n;
+      for (int c = lane; c < BN; c += 32) {
+        const int nn = n0 + c;
+        if (nn >= a.N) break;
+        float acc = 0.f;
+        for (int qq = 0; qq < S; ++qq) acc += *cl.map_shared_rank(P + rr * PP + c, qq);
+        if (a.mode == 0) {
+          const long long idx = (long long)m * a.N + nn;
+          float dv;
+          if (GDB && a.tangent == 2) dv = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
+          else dv = __ldg(a.D + idx);
+          const float x = acc + dv;
+          float z = x > 0.f ? x : a.alpha * x;
+          if constexpr (GDB) {
+            if (a.tangent == 1) z = (dv > 0.f ? 1.f : a.alpha) * acc;
+            else if (a.tangent == 2) z = (__ldg(a.Zmask + idx) > 0.f ? 1.f : a.alpha) * x;
           }
-          umma_commit(&empty[s]);  // stage free once these MMAs have read it
-        }
-        umma_commit(&acc_full[set]);   // chunk complete in accumulator set `set`
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---- epilogue: TMEM -> registers -> shared-memory transpose -> fused epilogue -> global ----
-    // tcgen05.ld gives every thread one ROW of the tile; global traffic wants one row per WARP
-    // instruction (lanes = consecutive columns).  Each epilogue warp transposes 32x32 chunks through
-    // a padded tile carved out of the (now idle) stage-0 operand buffer.
-    const int q = warp & 3;               // TMEM lane quarter this warp may access
-    // running sums of this thread's row (TMEM lane) in FP32 registers, round-to-nearest adds
-    float run[BN];
-#pragma unroll
-    for (int j = 0; j < BN; ++j) run[j] = 0.f;
-    {
-      const int nch = (nkb + a.ch - 1) / a.ch;
-      for (int c = 0; c < nch; ++c) {
-        const int set = c % TC_SETS;
-        mbar_wait(&acc_full[set], (uint32_t)((c / TC_SETS) & 1));
-        tc_fence_after();
-#pragma unroll
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(set * BN + c0), v);   // hi*hi of this chunk
-#pragma unroll
-          for (int j = 0; j < 32; ++j) run[c0 + j] += __uint_as_float(v[j]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[set]);
-      }
-      if (nch > 0) {   // the last acc_full commit covers every MMA issued before it: the cross-term accumulator is final
-#pragma unroll
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t w[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(TC_SETS * BN + c0), w);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) run[c0 + j] += __uint_as_float(w[j]);
-        }
-      }
-    }
-    float* tile = reinterpret_cast<float*>(smem) + q * (32 * 33);
-    // bundle-slot row pointer of the row this lane would own (backward mode), broadcast by shuffle
-    unsigned long long growp = 0;
-    if (a.mode == 1) {
-      const int mr = m0 + q * 32 + lane;
-      if (mr < a.M) {
-        float* gp = (a.perm == nullptr) ? a.g + (long long)mr * a.g_row_stride
-                                        : a.g + ((long long)mr * a.KS + a.perm[(long long)mr * a.KS + a.count[mr]]) * a.n;
-        growp = reinterpret_cast<unsigned long long>(gp);
-      }
-    }
-    if (S > 1) {
-      // ---- split-K epilogue: partial tile -> shared memory -> DSMEM sum -> fused epilogue ----
-      // (every CTA of the cluster reaches both cluster barriers: warps 0/1 call them below)
-      float* P = reinterpret_cast<float*>(smem);                  // [128][BN + 1] floats in the idle ring
-      constexpr int PP = BN + 1;
-#pragma unroll
-      for (int j = 0; j < BN; ++j) P[(q * 32 + lane) * PP + j] = run[j];
-      tc_fence_before();
-      cg::this_cluster().sync();
-      cg::cluster_group cl = cg::this_cluster();
-      const int rank = (int)cl.block_rank();
-      const int rlo = (TC_BM * rank) / S, rhi = (TC_BM * (rank + 1)) / S;
-      for (int rr = rlo + q; rr < rhi; rr += 4) {                // this warp's rows of the CTA's row slice
-        const int m = m0 + rr;
-        if (m >= a.M) break;
-        float* grow = nullptr;
-        if (a.mode == 1)
-          grow = (a.perm == nullptr) ? a.g + (long long)m * a.g_row_stride
-                                     : a.g + ((long long)m * a.KS + a.perm[(long long)m * a.KS + a.count[m]]) * a.n;
-        for (int c = lane; c < BN; c += 32) {
-          const int nn = n0 + c;
-          if (nn >= a.N) break;
-          float acc = 0.f;
-          for (int qq = 0; qq < S; ++qq) acc += *cl.map_shared_rank(P + rr * PP + c, qq);
-          if (a.mode == 0) {
-            const long long idx = (long long)m * a.N + nn;
-            float dv;
-            if (GDB && a.tangent == 2) dv = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
-            else dv = __ldg(a.D + idx);
-            const float x = acc + dv;
-            float z = x > 0.f ? x : a.alpha * x;
+          a.Z[idx] = z;
+          if (a.nxt_hi) {
+            const float p = z * __ldg(a.Cz_next + idx);
+            const float h = tf32_hi(p);
+            a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
+            a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
+          }
+        } else {
+          if (nn < a.N0) {
+            const long long idx = (long long)m * a.N0 + nn;
+            const float da = __ldg(a.Zprev + idx) > 0.f ? 1.f : a.alpha;
+            const float p = da * __ldg(a.Cz + idx) * acc;
+            const float h = tf32_hi(p);
+            a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
+            a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
             if constexpr (GDB) {
-              if (a.tangent == 1) z = (dv > 0.f ? 1.f : a.alpha) * acc;
-              else if (a.tangent == 2) z = (__ldg(a.Zmask + idx) > 0.f ? 1.f : a.alpha) * x;
-            }
-            a.Z[idx] = z;
-            if (a.nxt_hi) {
-              const float p = z * __ldg(a.Cz_next + idx);
-              const float h = tf32_hi(p);
-              a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
-              a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
+              if (a.dprev_plain) a.dprev_plain[idx] = p;
+              if (a.acc_plain) a.acc_plain[idx] = acc;
+              if (a.dCz) a.dCz[idx] = fmaf(a.kappa * __ldg(a.Ztprev + idx), acc, a.dCz[idx]);
+              if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, a.Dacc[idx]);
             }
           } else {
-            if (nn < a.N0) {
-              const long long idx = (long long)m * a.N0 + nn;
-              const float da = __ldg(a.Zprev + idx) > 0.f ? 1.f : a.alpha;
-              const float p = da * __ldg(a.Cz + idx) * acc;
-              const float h = tf32_hi(p);
-              a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
-              a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
-              if constexpr (GDB) {
-                if (a.dprev_plain) a.dprev_plain[idx] = p;
-                if (a.acc_plain) a.acc_plain[idx] = acc;
-                if (a.dCz) a.dCz[idx] = fmaf(a.kappa * __ldg(a.Ztprev + idx), acc, a.dCz[idx]);
-                if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, a.Dacc[idx]);
-              }
-            } else {
-              const int e = nn - a.N0;
-              grow[e] = fmaf(a.g_scale * __ldg(a.Cy + (long long)m * a.n + e), acc, grow[e]);
-            }
+            const int e = nn - a.N0;
+            grow[e] = fmaf(a.g_scale * __ldg(a.Cy + (long long)m * a.n + e), acc, grow[e]);
           }
         }
       }
-      cg::this_cluster().sync();   // partial tiles stay alive until every rank has read them
-    } else
+    }
+    cg::this_cluster().sync();   // partial tiles stay alive until every rank has read them
+    return;
+  }
+  __syncwarp();   // each warp reads back only the rows it wrote
+  // bundle-slot row pointer of row 16 warp + lane (backward mode, lanes 0..15), broadcast by shuffle
+  unsigned long long growp = 0;
+  if (a.mode == 1 && lane < 16) {
+    const int mr = m0 + warp * 16 + lane;
+    if (mr < a.M) {
+      float* gp = (a.perm == nullptr) ? a.g + (long long)mr * a.g_row_stride
+                                      : a.g + ((long long)mr * a.KS + a.perm[(long long)mr * a.KS + a.count[mr]]) * a.n;
+      growp = reinterpret_cast<unsigned long long>(gp);
+    }
+  }
 #pragma unroll
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      if (n0 + c0 >= a.N) break;          // warp-uniform: whole chunk out of range
+  for (int c0 = 0; c0 < BN; c0 += 32) {
+    if (n0 + c0 >= a.N) break;          // warp-uniform: whole chunk out of range
+    const int nn = n0 + c0 + lane;                     // this lane's column for the whole chunk
+    const bool nv = nn < a.N;
+    // rows in groups of RG: issue every global load of the group first (they are independent
+    // and L2-latency bound), then compute and store
+    constexpr int RG = 8;
+    for (int r0 = 0; r0 < 16; r0 += RG) {
+      if (m0 + warp * 16 + r0 >= a.M) break;           // warp-uniform
+      float acc[RG], in0[RG], in1[RG];
+      float in2[GDB ? RG : 1], in3[GDB ? RG : 1], in4[GDB ? RG : 1];
+      unsigned long long gp[RG];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) tile[lane * 33 + j] = run[c0 + j];
-      __syncwarp();
-      const int nn = n0 + c0 + lane;                     // this lane's column for the whole chunk
-      const bool nv = nn < a.N;
-      // rows in groups of RG: issue every global load of the group first (they are independent
-      // and L2-latency bound with only four epilogue warps per SM), then compute and store
-      // (RG = 16 measured slower on every workload: 160+ registers, C3 8.69 -> 8.89 ms, T 14.04 -> 14.28 ms)
-      constexpr int RG = 8;
-      for (int r0 = 0; r0 < 32; r0 += RG) {
-        if (m0 + q * 32 + r0 >= a.M) break;              // warp-uniform
-        float acc[RG], in0[RG], in1[RG];
-        float in2[GDB ? RG : 1], in3[GDB ? RG : 1], in4[GDB ? RG : 1];
-        unsigned long long gp[RG];
-#pragma unroll
-        for (int i = 0; i < RG; ++i) {
-          const int m = m0 + q * 32 + r0 + i;
-          acc[i] = tile[(r0 + i) * 33 + lane];
-          gp[i] = __shfl_sync(0xffffffffu, growp, r0 + i);
-          in0[i] = 0.f; in1[i] = 0.f;
-          if (nv && m < a.M) {
-            if (a.mode == 0) {
-              const long long idx = (long long)m * a.N + nn;
-              if (GDB && a.tangent == 2) {
-                in0[i] = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
-                in1[i] = __ldg(a.Zmask + idx);
-              } else {
-                in0[i] = __ldg(a.D + idx);
-                if (a.nxt_hi) in1[i] = __ldg(a.Cz_next + idx);
-              }
-            } else if (a.mode == 3) {
-              in0[i] = __ldg(a.bias + nn);
-            } else if (a.mode == 1) {
-              if (nn < a.N0) {
-                const long long idx = (long long)m * a.N0 + nn;
-                in0[i] = __ldg(a.Zprev + idx);
-                in1[i] = __ldg(a.Cz + idx);
-                if constexpr (GDB) {
-                  if (a.dCz) { in2[i] = __ldg(a.Ztprev + idx); in3[i] = a.dCz[idx]; }
-                  if (a.Dacc) in4[i] = a.Dacc[idx];
-                }
-              } else {
-                const int e = nn - a.N0;
-                in0[i] = __ldg(a.Cy + (long long)m * a.n + e);
-                in1[i] = reinterpret_cast<const float*>(gp[i])[e];
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < RG; ++i) {
-          const int m = m0 + q * 32 + r0 + i;
-          if (!nv || m >= a.M) continue;
+      for (int i = 0; i < RG; ++i) {
+        const int m = m0 + warp * 16 + r0 + i;
+        acc[i] = P[(warp * 16 + r0 + i) * PP + c0 + lane];
+        gp[i] = __shfl_sync(0xffffffffu, growp, r0 + i);
+        in0[i] = 0.f; in1[i] = 0.f;
+        if (nv && m < a.M) {
           if (a.mode == 0) {
             const long long idx = (long long)m * a.N + nn;
-            const float x = acc[i] + in0[i];
-            float z = x > 0.f ? x : a.alpha * x;
-            if constexpr (GDB) {
-              if (a.tangent == 1) z = (in0[i] > 0.f ? 1.f : a.alpha) * acc[i];
-              else if (a.tangent == 2) z = (in1[i] > 0.f ? 1.f : a.alpha) * x;
-            }
-            a.Z[idx] = z;
-            if (a.nxt_hi) {
-              const float p = z * in1[i];
-              const float h = tf32_hi(p);
-              a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
-              a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
-            }
-          } else if (a.mode == 1) {
-            if (nn < a.N0) {
-              const float da = in0[i] > 0.f ? 1.f : a.alpha;
-              const float p = da * in1[i] * acc[i];
-              const float h = tf32_hi(p);
-              a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
-              a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
-              if constexpr (GDB) {
-                const long long idx = (long long)m * a.N0 + nn;
-                if (a.dprev_plain) a.dprev_plain[idx] = p;
-                if (a.acc_plain) a.acc_plain[idx] = acc[i];
-                if (a.dCz) a.dCz[idx] = fmaf(a.kappa * in2[i], acc[i], in3[i]);
-                if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, in4[i]);
-              }
+            if (GDB && a.tangent == 2) {
+              in0[i] = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
+              in1[i] = __ldg(a.Zmask + idx);
             } else {
-              const int e = nn - a.N0;
-              reinterpret_cast<float*>(gp[i])[e] = fmaf(a.g_scale * in0[i], acc[i], in1[i]);
+              in0[i] = __ldg(a.D + idx);
+              if (a.nxt_hi) in1[i] = __ldg(a.Cz_next + idx);
             }
           } else if (a.mode == 3) {
-            int r = 0;
-#pragma unroll
-            for (int t = 1; t < 4; ++t) if (t < a.nr && nn >= a.rbeg[t]) r = t;
-            float v = acc[i] + in0[i];
-            if (a.rrelu[r]) v = fmaxf(v, 0.f);
-            const int c = nn - a.rbeg[r];
-            if (r == 0 && a.r0_hi) {
-              const float h = tf32_hi(v);
-              a.r0_hi[(long long)m * a.rld[0] + c] = h;
-              a.r0_lo[(long long)m * a.rld[0] + c] = tf32_lo(v, h);
+            in0[i] = __ldg(a.bias + nn);
+          } else if (a.mode == 1) {
+            if (nn < a.N0) {
+              const long long idx = (long long)m * a.N0 + nn;
+              in0[i] = __ldg(a.Zprev + idx);
+              in1[i] = __ldg(a.Cz + idx);
+              if constexpr (GDB) {
+                if (a.dCz) { in2[i] = __ldg(a.Ztprev + idx); in3[i] = a.dCz[idx]; }
+                if (a.Dacc) in4[i] = a.Dacc[idx];
+              }
             } else {
-              a.rdst[r][(long long)m * a.rld[r] + c] = v;
+              const int e = nn - a.N0;
+              in0[i] = __ldg(a.Cy + (long long)m * a.n + e);
+              in1[i] = reinterpret_cast<const float*>(gp[i])[e];
             }
-          } else {
-            a.C[(long long)m * a.N + nn] = acc[i];
           }
         }
       }
-      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < RG; ++i) {
+        const int m = m0 + warp * 16 + r0 + i;
+        if (!nv || m >= a.M) continue;
+        if (a.mode == 0) {
+          const long long idx = (long long)m * a.N + nn;
+          const float x = acc[i] + in0[i];
+          float z = x > 0.f ? x : a.alpha * x;
+          if constexpr (GDB) {
+            if (a.tangent == 1) z = (in0[i] > 0.f ? 1.f : a.alpha) * acc[i];
+            else if (a.tangent == 2) z = (in1[i] > 0.f ? 1.f : a.alpha) * x;
+          }
+          a.Z[idx] = z;
+          if (a.nxt_hi) {
+            const float p = z * in1[i];
+            const float h = tf32_hi(p);
+            a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
+            a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
+          }
+        } else if (a.mode == 1) {
+          if (nn < a.N0) {
+            const float da = in0[i] > 0.f ? 1.f : a.alpha;
+            const float p = da * in1[i] * acc[i];
+            const float h = tf32_hi(p);
+            a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
+            a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
+            if constexpr (GDB) {
+              const long long idx = (long long)m * a.N0 + nn;
+              if (a.dprev_plain) a.dprev_plain[idx] = p;
+              if (a.acc_plain) a.acc_plain[idx] = acc[i];
+              if (a.dCz) a.dCz[idx] = fmaf(a.kappa * in2[i], acc[i], in3[i]);
+              if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, in4[i]);
+            }
+          } else {
+            const int e = nn - a.N0;
+            reinterpret_cast<float*>(gp[i])[e] = fmaf(a.g_scale * in0[i], acc[i], in1[i]);
+          }
+        } else if (a.mode == 3) {
+          int r = 0;
+#pragma unroll
+          for (int t = 1; t < 4; ++t) if (t < a.nr && nn >= a.rbeg[t]) r = t;
+          float v = acc[i] + in0[i];
+          if (a.rrelu[r]) v = fmaxf(v, 0.f);
+          const int c = nn - a.rbeg[r];
+          if (r == 0 && a.r0_hi) {
+            const float h = tf32_hi(v);
+            a.r0_hi[(long long)m * a.rld[0] + c] = h;
+            a.r0_lo[(long long)m * a.rld[0] + c] = tf32_lo(v, h);
+          } else {
+            a.rdst[r][(long long)m * a.rld[r] + c] = v;
+          }
+        } else {
+          a.C[(long long)m * a.N + nn] = acc[i];
+        }
+      }
     }
-    tc_fence_before();
-  }
-  if (S > 1 && warp < 2) { cg::this_cluster().sync(); cg::this_cluster().sync(); }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 4 * BN);
   }
 }
 
@@ -651,7 +626,7 @@ static cudaError_t launch_tc_variant(const CUtensorMap& tAh, const CUtensorMap& 
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(cdiv(a.N, BN), cdiv(a.M, TC_BM), splitk);
-  cfg.blockDim = dim3(192);
+  cfg.blockDim = dim3(TC_THREADS);
   cfg.dynamicSmemBytes = TcSmem<BN, NST_>::TOTAL;
   cfg.stream = st;
   cudaLaunchAttribute lattr[1];
@@ -667,9 +642,8 @@ static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const
   // tile choice: 64-wide tiles; two CTAs per SM (the epilogue of one overlaps the main loop of the
   // other) once there are >= 2 tiles per SM, else one CTA per SM with a 4-deep ring.
   // ICNN_TC_CFG=128|64x4|64x2 forces a variant.
-  // (measured on B200, T shape: 64x2 4.28 ms, 128 5.12 ms, 64x4 6.62 ms per 10 iterations of K1;
-  //  C2, 28 tiles: 64x4 7.5 ms, 64x2 8.0 ms, 128 9.2 ms)
-  int cfg = (cdiv(a.N, 64) * gy >= 296) ? 2 : 1;
+  const int sms = device_sms();
+  int cfg = (cdiv(a.N, 64) * gy >= 2 * sms) ? 2 : 1;
   static const int env_cfg = [] {     // tuning knobs are read once per process, not per launch
     const char* v = getenv("ICNN_TC_CFG");
     if (!v) return -1;
@@ -699,7 +673,7 @@ static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const
   int splitk = 1;
   if (cfg == 1 && (a.mode == 0 || a.mode == 1)) {
     const int tiles = cdiv(a.N, 64) * gy, nkb = cdiv(a.K, TC_BK);
-    while (splitk < 8 && tiles * splitk * 2 <= 148 && nkb / (splitk * 2) >= 4) splitk *= 2;
+    while (splitk < 8 && tiles * splitk * 2 <= sms && nkb / (splitk * 2) >= 4) splitk *= 2;
     if (env_splitk) splitk = env_splitk;
   }
   cudaError_t e;

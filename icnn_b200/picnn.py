@@ -84,7 +84,7 @@ class PICNN:
             stream = torch.cuda.current_stream().cuda_stream
             _capi.check(_capi.lib.icnn_picnn_create(C.byref(desc), C.byref(handle), C.c_void_p(stream)))
         self._h = handle
-        # x-path gate precompute on the library's tcgen05 GEMM when the shapes allow it
+        # x-path gate precompute on the library's wgmma GEMM when the shapes allow it
         # (SURVEY.md section 8f row 2); otherwise plain cuBLAS GEMMs through torch.addmm
         self._xpath = False
         with torch.cuda.device(self.device):
@@ -136,7 +136,7 @@ class PICNN:
         return torch.empty(max(nbytes, 4), dtype=torch.uint8, device=self.device)
 
     def gates(self, x):
-        """x-path products (cz, cy, d), constant over the inner loop (SURVEY.md section 8f row 2): one tcgen05 GEMM per
+        """x-path products (cz, cy, d), constant over the inner loop (SURVEY.md section 8f row 2): one wgmma GEMM per
         source activation with a bias / ReLU / scatter epilogue (``icnn_picnn_gates``).  Only when the library reports
         the shape unsupported (``icnn_picnn_set_xpath`` -> ICNN_E_UNSUPPORTED, e.g. ICNN_K1=simt builds of the handle)
         the same products are formed by library GEMMs (torch.addmm -> cuBLAS): a once-per-solveBatch precompute,

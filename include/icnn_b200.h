@@ -1,10 +1,10 @@
 /*
- * icnn_b200 -- C ABI of the B200-native ICNN inner-loop library (libicnn_b200.so).
+ * icnn_b200 -- C ABI of the H100-native ICNN inner-loop library (libicnn_b200.so).
  *
  * Drop-in boundary for ONE hot path of locuslab/icnn: argmin_y f(x, y; theta) by the
  * bundle-entropy method and by unrolled momentum gradient descent.  The reference is pure
  * Python/numpy/TensorFlow and has no FFI of its own; each entry point below names the reference
- * function (path:line under /root/reference) whose work it replaces.  The Python side
+ * function (path:line in the locuslab/icnn repository) whose work it replaces.  The Python side
  * (icnn_b200/_capi.py, ctypes) is the binding a maintainer of the reference would add -- see
  * INTEGRATION.md.
  *
@@ -151,7 +151,7 @@ int icnn_picnn_fg(const icnn_picnn_t* h, const icnn_gates* gates, const float* y
  * (multi-label-cls/icnn_ebundle.py:339-347,354-356,363-365,372-373), evaluated once per solveBatch.
  * set_xpath hands the library the x-path weights (host arrays of device pointers, [in, out] layout;
  * Wu/bu: L entries, the others L+1, Wzu[0]/bzu[0] ignored); gates() then fills cz/cy/d for a
- * minibatch x [B, m] with one tcgen05 GEMM per source activation (bias, ReLU and the scatter into
+ * minibatch x [B, m] with one wgmma GEMM per source activation (bias, ReLU and the scatter into
  * the outputs fused into the epilogue).  ICNN_E_UNSUPPORTED when a width is not a multiple of 4. */
 int icnn_picnn_set_xpath(icnn_picnn_t* h, int32_t m, const float* const* Wu, const float* const* bu,
                          const float* const* Wzu, const float* const* bzu, const float* const* Wyu,
@@ -244,7 +244,7 @@ int icnn_adam_solve(const icnn_picnn_t* h, const icnn_gates* gates, double* act_
                     int32_t max_iter, int32_t* iters_out, void* scratch, void* workspace, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------ */
-/* Self test of the tcgen05 / TMA GEMM the tensor-core K1 path is built from:
+/* Self test of the wgmma / TMA GEMM the tensor-core K1 path is built from:
  * C[M,N] = A[M,K] * B[N,K]^T with the 3xTF32 split (all row-major device buffers, K % 4 == 0;
  * scratch holds 2*M*K + 2*N*K floats). */
 int icnn_tc_gemm_selftest(const float* A, const float* B, float* C, int32_t M, int32_t N, int32_t K,

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py): the checker for the CUDA path and the timed
 CPU baseline of bench.py.  Written from the algorithms in SURVEY.md Appendix C, following
-(paths relative to /root/reference):
+(paths relative to the locuslab/icnn repository):
 
   variant 'lib'  : lib/bundle_entropy.py        solveBatch :192-242, pdipm_pc :5-78,
                                                  pdipm_boyd :80-156, get_step :158-163

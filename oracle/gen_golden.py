@@ -1,12 +1,11 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the UNMODIFIED reference modules.
 
-TEST INFRASTRUCTURE ONLY.  Runs only in the build container (needs /root/reference, which is
-absent on the GPU box); the committed .npz files are what travels.  The three reference files
-import unchanged under numpy/scipy:
-    /root/reference/lib/bundle_entropy.py        (solveBatch, solver='pc' / 'boyd')
-    /root/reference/lib/bundle_entropy_dual.py   (solveBatch)
-    /root/reference/RL/src/bundle_entropy.py     (solveBatch)
+TEST INFRASTRUCTURE ONLY.  Needs a checkout of the reference (locuslab/icnn) at $ICNN_REFERENCE_DIR;
+the tests read only the committed .npz files.  The three reference files import unchanged under numpy/scipy:
+    lib/bundle_entropy.py        (solveBatch, solver='pc' / 'boyd')
+    lib/bundle_entropy_dual.py   (solveBatch)
+    RL/src/bundle_entropy.py     (solveBatch)
 The PICNN f/g callback they are fed is oracle/picnn_np.py (the reference's own f is a
 TensorFlow graph and TensorFlow is not installed) in float64; inputs are regenerated from the
 seed by oracle/synth.py, and a checksum of the inputs is stored so generator drift is caught.
@@ -27,7 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import picnn_np, synth  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("ICNN_REFERENCE_DIR", "")
 
 
 def _load(name, path):

@@ -3,7 +3,7 @@
 produced by EXECUTING THE REFERENCE'S OWN graph code (cut out of its files with ``ast``, unmodified) on
 oracle/tf_shim.py -- TensorFlow / tflearn are not installed, the shim restates only their primitives.
 
-Executed reference code (paths under /root/reference):
+Executed reference code (paths relative to a locuslab/icnn checkout):
   multi-label-cls/icnn_ebundle.py  class Model: __init__ (:120-166) and f (:316-388)  -> E_, dE_dy_
   multi-label-cls/icnn-back.py     class Model: __init__ (:104-147) and f (:233-305)  -> yn_, energies_, mse_,
                                    opt.compute_gradients(mse_, theta_)
@@ -18,7 +18,7 @@ oracle/gd_grad_np.py (training gradient through the unrolled loop) -- tests/test
 compared with the device kernels in tests/test_gpu_picnn.py.  Weights and inputs are regenerated from seeds by
 ``case_inputs`` (shared with the tests); only outputs are stored.
 
-TEST INFRASTRUCTURE ONLY; runs in the build container only (needs /root/reference).
+TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
 Usage:  python oracle/gen_golden_tfshim.py
 """
 import ast
@@ -34,7 +34,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from icnn_b200 import workloads  # noqa: E402  (pure-numpy input generator)
 
-REF = "/root/reference"
+REF = os.environ.get("ICNN_REFERENCE_DIR", "")
 BN_EPS = 1e-5
 
 
@@ -276,7 +276,7 @@ def run_completion_model(tag):
 
 
 def generate():
-    """-> {name: array}: every golden of tests/golden/picnn_tfshim.npz, recomputed from /root/reference."""
+    """-> {name: array}: every golden of tests/golden/picnn_tfshim.npz, recomputed from the reference checkout."""
     sys.path.insert(0, os.path.join(REF, "RL", "src"))
     from oracle.gen_golden import _load
     out = {}

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  The reference builds this fu
 TensorFlow graph (TensorFlow/tflearn absent here), so it is restated from the cited lines; tflearn
 ``fully_connected`` is ``out = in @ W + b`` with W laid out ``[in, out]``.
 
-Follows (paths relative to /root/reference):
+Follows (paths relative to the locuslab/icnn repository):
   * multi-label-cls/icnn_ebundle.py:316-388  (Model.f: ReLU PICNN, ``nLabels`` appended to szs)
   * RL/src/icnn.py:325-404                   (Agent.negQ: leaky-ReLU PICNN, szs = [l1, l2])
   * multi-label-cls/icnn_ebundle.py:146      (dE_dy_ = tf.gradients(E_, y_))

@@ -95,7 +95,7 @@ def test_device_list_environment_variable(monkeypatch):
 
 def test_plain_c_consumer_compiles_and_links_without_a_gpu(tmp_path):
     """include/icnn_b200.h is valid C99 (no C++-isms, no torch types) and tests/c_abi/smoke.c -- the plain-C consumer
-    the GPU suite runs -- compiles and links against libicnn_b200.so here (it is executed on the GPU box only)."""
+    the GPU suite runs -- compiles and links against libicnn_b200.so here (it is executed by the GPU test only)."""
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     hdr_only = tmp_path / "hdr.c"

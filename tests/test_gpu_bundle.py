@@ -24,13 +24,13 @@ np.seterr(all="ignore")
 
 
 def _parity_record(key, d, floor, extra=None):
-    """Append the per-config parity statistics to gpurun_out/r02_parity_raw.json (copied to
-    profiles/r02_parity.json by hand after a GPU run; a missing directory is not an error)."""
+    """Append the per-config parity statistics to $ICNN_PARITY_DIR/parity_raw.json when that directory is set
+    and exists (nothing is written otherwise)."""
     import json
-    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
-    if not os.path.isdir(out):
+    out = os.environ.get("ICNN_PARITY_DIR")
+    if not out or not os.path.isdir(out):
         return
-    path = os.path.join(out, "r02_parity_raw.json")
+    path = os.path.join(out, "parity_raw.json")
     try:
         with open(path) as f:
             data = json.load(f)
@@ -185,7 +185,7 @@ def test_k2_against_reference_golden(case, maxtol, medtol, golden_dir):
         assert agree >= (0.5 if nIter > 10 else 0.8), agree
 
 
-# ("T", 160, ...) and ("C2", 70, ...) have >= 64 rows: K1 and the gate precompute run on the tcgen05 path
+# ("T", 160, ...) and ("C2", 70, ...) have >= 64 rows: K1 and the gate precompute run on the wgmma path
 FUSED = [("C1", 64, 5, 1e-4), ("C4", 512, 5, 1e-4), ("T", 48, 10, 1e-4), ("T", 160, 10, None), ("C3", 96, 10, None),
          ("C2", 6, 30, None), ("C2", 70, 8, None)]
 
@@ -230,7 +230,7 @@ def test_shard_concat_equals_unsharded(name, B, cut, nIter):
     """Samples are independent: solving two row blocks separately equals solving the batch at
     once (what the multi-GPU sharding relies on) -- up to float32 summation order in K1, whose
     split-K factor follows the grid size.  Both shards keep >= 64 rows (same K1 path), and the horizons are
-    the ones where the float32 noise floor of the workload is below 1 % (profiles/r02_parity.json), so that a
+    the ones where the float32 noise floor of the workload is below 1 %, so that a
     disagreement would be a sharding bug and not a ReLU-kink flip."""
     import icnn_b200
     from icnn_b200 import bundle_entropy as be

@@ -1,10 +1,9 @@
 """d mse / d theta through the unrolled momentum-GD loop (multi-label-cls/icnn-back.py:116-139) on the
 GPU vs the torch-autograd golden vectors and the float64 numpy restatement.
 
-Tolerance: the device path is float32 (3xTF32 tcgen05 or FFMA GEMMs, float32 accumulation over the
+Tolerance: the device path is float32 (3xTF32 wgmma or FFMA GEMMs, float32 accumulation over the
 batch and the nIter iterations); every gradient array must agree with the float64 reference to 2e-4
-of that array's largest entry on the samples whose iterates cross no ReLU kink differently
-(measured 1e-6 .. 5e-5: profiles/r01_gd_grad.md)."""
+of that array's largest entry on the samples whose iterates cross no ReLU kink differently."""
 import os
 
 import numpy as np

@@ -2,7 +2,7 @@
 REFERENCE'S OWN graph code (multi-label-cls/icnn_ebundle.py Model.__init__/f, multi-label-cls/icnn-back.py
 Model.__init__/f, RL/src/icnn.py Agent.negQ / Agent.bundle_entropy) executed unmodified on the TensorFlow /
 tflearn stand-in oracle/tf_shim.py by oracle/gen_golden_tfshim.py.  CPU only; the golden file and the seeded
-inputs travel, /root/reference is not read here."""
+inputs are all it needs."""
 import os
 
 import numpy as np
@@ -158,20 +158,3 @@ def test_conv_picnn_helper_matches_the_reference_graph(tag, gold):
     close(f, gold[tag + "_f"], "E_")
     close(g, gold[tag + "_g"], "dE_dy_")
 
-
-@pytest.mark.skipif(not os.path.isdir("/root/reference/multi-label-cls"), reason="needs the reference checkout (build container only)")
-def test_committed_goldens_regenerate_from_the_reference(gold):
-    """The committed vectors ARE what the reference's code produces on the stand-in: re-run the generator here
-    (the build container holds /root/reference; the GPU box does not, and skips this) and compare every array."""
-    import contextlib
-    import io
-    from oracle import gen_golden_tfshim
-    with contextlib.redirect_stdout(io.StringIO()):
-        fresh = gen_golden_tfshim.generate()
-    assert sorted(fresh) == sorted(gold.files)
-    for k in gold.files:
-        a, b = np.asarray(fresh[k]), gold[k]
-        if a.dtype.kind in "US":
-            assert list(a) == list(b), k
-        else:
-            close(a, b, k, rtol=1e-12)

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Markdown table of a bench.py JSON line (headline + configs sub-records): python tools/bench_table.py profiles/X.json"""
+"""Markdown table of a bench.py JSON line (headline + configs sub-records): python tools/bench_table.py bench_line.json
+(a file holding the line bench.py printed)"""
 import json
 import sys
 

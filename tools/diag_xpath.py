@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0,'/root/repo')
+import os, sys; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, icnn_b200
 from oracle import picnn_np, synth
 for B in (5, 40, 64, 130):

@@ -1,8 +1,8 @@
 """Small end-to-end cases for compute-sanitizer (memcheck / racecheck / synccheck):
     compute-sanitizer --tool racecheck python tools/sanitize_case.py
-Covers K1 FFMA + cluster split-K, K1 tcgen05 path, K2 group kernel (WPS 1/2/8, PC + dual + RL Newton),
-K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the tcgen05 path (pitch-padded
-operands), GD training backward (FFMA and tcgen05 GDB instantiation, split-K weight-gradient GEMM)."""
+Covers K1 FFMA + cluster split-K, K1 wgmma path, K2 group kernel (WPS 1/2/8, PC + dual + RL Newton),
+K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the wgmma path (pitch-padded
+operands), GD training backward (FFMA and wgmma GDB instantiation, split-K weight-gradient GEMM)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -49,7 +49,7 @@ if "gdgrad" in which:
                                            nIter=3, lr=0.02, momentum=0.5, x=x)
         print("gdgrad ok", dims, B, float(np.abs(gr["Wy"][0]).max()), flush=True)
 if "pc" in which:     # round 2: the two-sweep PC kernel in every group size, both alignments, the > 4 row-block sweeps, and
-    # the chunked-accumulation tcgen05 GEMM (T, 64 rows above)
+    # the chunked-accumulation wgmma GEMM (T, 64 rows above)
     run("C3", 5, 5)                                     # 1 warp / sample, n_y % 4 != 0 (scalar row loads)
     for w in ("1", "2", "4", "8"):
         os.environ["ICNN_PC_WPS"] = w

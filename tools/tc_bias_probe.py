@@ -1,4 +1,4 @@
-"""Signed error of the tcgen05 3xTF32 GEMM (C = A B^T) vs float64: is the systematic bias a function of the
+"""Signed error of the wgmma 3xTF32 GEMM (C = A B^T) vs float64: is the systematic bias a function of the
 accumulation LENGTH (then slicing K helps) or intrinsic to every MMA (then it does not)?"""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

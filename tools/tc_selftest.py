@@ -1,4 +1,4 @@
-"""tcgen05 / TMA 3xTF32 GEMM self test: C = A B^T vs float64, several shapes."""
+"""wgmma / TMA 3xTF32 GEMM self test: C = A B^T vs float64, several shapes."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
