@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 NSTAT = 8
 
 # status / enum mirrors of include/icnn_b200.h
@@ -31,6 +31,7 @@ SYMBOLS = [
     "icnn_adam_workspace_bytes", "icnn_adam_solve",
     "icnn_gd_backward_workspace_bytes", "icnn_gd_backward", "icnn_fp64_mma_probe",
     "icnn_loop_graph_create", "icnn_loop_graph_launch", "icnn_loop_graph_nodes", "icnn_loop_graph_destroy",
+    "icnn_tc_set_tuning", "icnn_tc_last_launch",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -96,6 +97,8 @@ def _load():
                                   C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
     lib.icnn_tc_gemm_selftest.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_void_p, C.c_void_p]
+    lib.icnn_tc_set_tuning.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    lib.icnn_tc_last_launch.argtypes = [C.POINTER(C.c_int32)]
     lib.icnn_picnn_set_xpath.argtypes = [C.c_void_p, C.c_int32] + [_fpp] * 8 + [C.c_void_p]
     lib.icnn_picnn_gates_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
     lib.icnn_picnn_gates_workspace_bytes.restype = C.c_size_t

@@ -51,6 +51,14 @@ __device__ __forceinline__ double neg_entropy(double y) {
   if (y < 1.0) a += (1.0 - y) * log(1.0 - y);
   return a;
 }
+// x rounded to nearest TF32 (10-bit mantissa, ties away from zero), the hi / lo split of the tensor-core operands.
+// Inf and NaN pass unchanged: the rounding carry would turn a NaN with high payload bits (0x7FFFFFFF, the NaN the
+// GPU's own arithmetic produces) into -0 or +0, and a product with it would silently come out finite.
+__device__ __forceinline__ float tf32_rn(float x) {
+  const uint32_t u = __float_as_uint(x);
+  if ((u & 0x7F800000u) == 0x7F800000u) return x;
+  return __uint_as_float((u + 0x00001000u) & 0xFFFFE000u);
+}
 #endif
 // leading dimension padded to 4 floats: 16-byte row pitch for TMA; the pad columns lie outside the
 // tensor map's extent (TMA zero-fills them), so they are never read and need no initialisation

@@ -220,10 +220,10 @@ __global__ void tangent_stage_kernel(StageArgs a) {
     if (a.As) {
       acc = fmaf(k * zt, a.As[off], acc);
       const float p = zt * czv;
-      const float h = __uint_as_float((__float_as_uint(p) + 0x00001000u) & 0xFFFFE000u);   // tf32_rn, as picnn_tc.cu
+      const float h = tf32_rn(p);
       const long long o = ((long long)i * a.B + b) * a.ldp + j;
       a.P_hi[o] = h;
-      a.P_lo[o] = __uint_as_float((__float_as_uint(p - h) + 0x00001000u) & 0xFFFFE000u);
+      a.P_lo[o] = tf32_rn(p - h);
       a.Pk[off] = k * p;
     } else {
       acc = fmaf(k, zt, acc);

@@ -50,11 +50,11 @@ __global__ void __launch_bounds__(256) out_layer_kernel(OutArgs a) {
       const float dl = (z > 0.f ? 1.f : a.alpha) * c;
       if (a.delta) a.delta[idx] = dl;
       if (a.delta_hi) {
-        // TF32 hi/lo with round-to-nearest on both parts (see tf32_rn in picnn_tc.cu)
-        const float h = __uint_as_float((__float_as_uint(dl) + 0x00001000u) & 0xFFFFE000u);
+        // TF32 hi/lo with round-to-nearest on both parts
+        const float h = tf32_rn(dl);
         const long long o = (long long)m * a.delta_ld + j;
         a.delta_hi[o] = h;
-        a.delta_lo[o] = __uint_as_float((__float_as_uint(dl - h) + 0x00001000u) & 0xFFFFE000u);
+        a.delta_lo[o] = tf32_rn(dl - h);
       }
     }
     float* grow;

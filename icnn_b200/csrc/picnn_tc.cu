@@ -23,6 +23,7 @@
 #include <cuda.h>
 #include <cooperative_groups.h>
 
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 
@@ -140,8 +141,7 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
 
 // TF32 split with round-to-nearest on both parts: hi = rn_tf32(x), lo = rn_tf32(x - hi), both exactly
 // representable in TF32 (the tensor core would otherwise TRUNCATE its inputs), so
-// |x - (hi + lo)| <= 2^-22 |x|  (measured: gates/f/g errors 2-4x lower than with truncation).
-__device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x00001000u) & 0xFFFFE000u); }
+// |x - (hi + lo)| <= 2^-22 |x|  (measured: gates/f/g errors 2-4x lower than with truncation).  tf32_rn: common.cuh
 __device__ __forceinline__ float tf32_hi(float x) { return tf32_rn(x); }
 __device__ __forceinline__ float tf32_lo(float x, float hi) { return tf32_rn(x - hi); }
 
@@ -359,7 +359,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
             a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
             a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
           }
-        } else {
+        } else if (a.mode == 2) {
+          a.C[(long long)m * a.N + nn] = acc;
+        } else if (a.mode == 1) {   // (mode 3 never launches split: launch_tc_gemm)
           if (nn < a.N0) {
             const long long idx = (long long)m * a.N0 + nn;
             const float da = __ldg(a.Zprev + idx) > 0.f ? 1.f : a.alpha;
@@ -636,12 +638,17 @@ static cudaError_t launch_tc_variant(const CUtensorMap& tAh, const CUtensorMap& 
   return cudaLaunchKernelEx(&cfg, tc_gemm_kernel<BN, NST_, GDB>, tAh, tAl, tBh, tBl, a);
 }
 
+// Process-wide tuning override (icnn_tc_set_tuning), applied on top of the environment knobs; -1 = automatic.
+static std::atomic<int> g_tc_cfg{-1}, g_tc_splitk{-1}, g_tc_ch{-1};
+// {BN, NST, splitk, ch, mode} of the calling thread's most recent launch_tc_gemm (icnn_tc_last_launch)
+static thread_local int g_tc_last[5] = {0, 0, 0, 0, -1};
+
 static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const float* Bh, const float* Bl, long long ldb,
                           TcArgs a, cudaStream_t st, bool gdb = false) {
   const int gy = cdiv(a.M, TC_BM);
   // tile choice: 64-wide tiles; two CTAs per SM (the epilogue of one overlaps the main loop of the
   // other) once there are >= 2 tiles per SM, else one CTA per SM with a 4-deep ring.
-  // ICNN_TC_CFG=128|64x4|64x2 forces a variant.
+  // ICNN_TC_CFG=128|64x4|64x2 or icnn_tc_set_tuning forces a variant.
   const int sms = device_sms();
   int cfg = (cdiv(a.N, 64) * gy >= 2 * sms) ? 2 : 1;
   static const int env_cfg = [] {     // tuning knobs are read once per process, not per launch
@@ -659,9 +666,13 @@ static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const
     const int w = v ? atoi(v) : 0;
     return (w >= 1 && w <= 64) ? w : TC_CH;
   }();
-  a.ch = env_ch;
+  const int ov_cfg = g_tc_cfg.load(std::memory_order_relaxed);
+  const int ov_splitk = g_tc_splitk.load(std::memory_order_relaxed);
+  const int ov_ch = g_tc_ch.load(std::memory_order_relaxed);
+  a.ch = ov_ch > 0 ? ov_ch : env_ch;
   if (env_cfg >= 0) cfg = env_cfg;
-  if (gdb && cfg == 0) cfg = 1;
+  if (ov_cfg >= 0) cfg = ov_cfg;
+  if (gdb && cfg == 0) cfg = 1;   // the GDB epilogue has no 128-wide instantiation
   const int BN = cfg == 0 ? 128 : 64;
   CUtensorMap tAh, tAl, tBh, tBl;
   int rc;
@@ -669,12 +680,14 @@ static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const
   if ((rc = make_tmap(&tAl, Al, a.M, a.K, lda, TC_BM))) return rc;
   if ((rc = make_tmap(&tBh, Bh, a.N, a.K, ldb, BN))) return rc;
   if ((rc = make_tmap(&tBl, Bl, a.N, a.K, ldb, BN))) return rc;
-  // split-K over a cluster when the tile grid leaves most of the chip idle (C2: 4 row tiles)
+  // split-K over a cluster when the tile grid leaves most of the chip idle (C2: 4 row tiles); only <64,4> and the
+  // modes the split-K epilogue implements (0, 1, 2; the mode-3 gate epilogue never splits)
   int splitk = 1;
-  if (cfg == 1 && (a.mode == 0 || a.mode == 1)) {
+  if (cfg == 1 && a.mode != 3) {
     const int tiles = cdiv(a.N, 64) * gy, nkb = cdiv(a.K, TC_BK);
     while (splitk < 8 && tiles * splitk * 2 <= sms && nkb / (splitk * 2) >= 4) splitk *= 2;
     if (env_splitk) splitk = env_splitk;
+    if (ov_splitk > 0) splitk = ov_splitk;
   }
   cudaError_t e;
   if (gdb)   // GD training backward: the 64-wide variants with the tangent / accumulation epilogue
@@ -685,6 +698,8 @@ static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const
       : cfg == 1 ? launch_tc_variant<64, 4>(tAh, tAl, tBh, tBl, a, splitk, st)
                  : launch_tc_variant<64, 2>(tAh, tAl, tBh, tBl, a, 1, st);
   if (e != cudaSuccess) { set_error("tc_gemm launch: %s", cudaGetErrorString(e)); return ICNN_E_CUDA; }
+  const int launched[5] = {BN, cfg == 0 ? 3 : cfg == 1 ? 4 : 2, splitk, a.ch, a.mode};
+  memcpy(g_tc_last, launched, sizeof(launched));
   return ICNN_OK;
 }
 
@@ -989,6 +1004,26 @@ extern "C" int icnn_picnn_gates(const icnn_picnn_t* h, const float* x, int32_t B
   ICNN_REQUIRE(B > 0, "empty batch");
   if (!h->has_xpath) { set_error("icnn_picnn_set_xpath was not called"); return ICNN_E_INVALID; }
   return picnn_gates_tc(h, x, B, cz, cy, d, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// Pins the tile variant / split-K factor / chunk length of every later tensor-core GEMM of the process (tests
+// reach each variant on any SM count); -1 restores the automatic choice.  A forced value only applies where the
+// launch can honour it: split-K needs <64,4> and a mode with a split-K epilogue, GDB maps <128,3> to <64,4>.
+extern "C" int icnn_tc_set_tuning(int32_t cfg, int32_t splitk, int32_t ch) {
+  ICNN_REQUIRE(cfg >= -1 && cfg <= 2, "cfg must be -1 (automatic), 0 (<128,3>), 1 (<64,4>) or 2 (<64,2>)");
+  ICNN_REQUIRE(splitk == -1 || splitk == 1 || splitk == 2 || splitk == 4 || splitk == 8,
+               "splitk must be -1 (automatic), 1, 2, 4 or 8");
+  ICNN_REQUIRE(ch == -1 || (ch >= 1 && ch <= 64), "ch must be -1 (default) or 1..64");
+  g_tc_cfg.store(cfg);
+  g_tc_splitk.store(splitk);
+  g_tc_ch.store(ch);
+  return ICNN_OK;
+}
+
+extern "C" int icnn_tc_last_launch(int32_t out[5]) {
+  ICNN_REQUIRE(out, "null pointer");
+  for (int i = 0; i < 5; ++i) out[i] = g_tc_last[i];
+  return ICNN_OK;
 }
 
 // Self test of the tensor-core GEMM: C[M,N] = A[M,K] * B[N,K]^T (3xTF32), all device, row-major.

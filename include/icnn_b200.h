@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ICNN_ABI_VERSION 3
+#define ICNN_ABI_VERSION 4
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -245,10 +245,21 @@ int icnn_adam_solve(const icnn_picnn_t* h, const icnn_gates* gates, double* act_
 
 /* ---- diagnostics ------------------------------------------------------------------------------ */
 /* Self test of the wgmma / TMA GEMM the tensor-core K1 path is built from:
- * C[M,N] = A[M,K] * B[N,K]^T with the 3xTF32 split (all row-major device buffers, K % 4 == 0;
- * scratch holds 2*M*K + 2*N*K floats). */
+ * C[M,N] = A[M,K] * B[N,K]^T with the 3xTF32 split (all row-major device buffers, any M, N, K >= 1;
+ * scratch holds (2*M + 2*N) * ((K + 3) & ~3) floats: the split operands, rows padded to 4 floats). */
 int icnn_tc_gemm_selftest(const float* A, const float* B, float* C, int32_t M, int32_t N, int32_t K,
                           float* scratch, void* stream);
+/* Pins the tensor-core GEMM's tuning for every later launch in the process (all threads), on top of the
+ * ICNN_TC_CFG / ICNN_TC_SPLITK / ICNN_TC_CH environment variables; -1 = automatic / default.
+ *   cfg: 0 = 128-wide tiles, 3-stage ring; 1 = 64-wide, 4 stages; 2 = 64-wide, 2 stages (two CTAs per SM)
+ *   splitk: 1, 2, 4 or 8 (applies only to cfg 1 and to the GEMMs with a split-K epilogue, not the x-path gates)
+ *   ch: 1..64 half k-blocks (K = 16 each) per round-to-nearest accumulation chunk
+ * The GD training backward has no 128-wide variant and runs cfg 0 as cfg 1.  Out-of-range values return
+ * ICNN_E_INVALID and leave the current setting unchanged. */
+int icnn_tc_set_tuning(int32_t cfg, int32_t splitk, int32_t ch);
+/* out (host, 5 int32) = {tile width BN, ring stages, split-K factor, chunk length, mode} of the calling thread's
+ * most recent tensor-core GEMM launch (mode 0 forward, 1 backward, 2 self test, 3 x-path gates; -1 = none yet). */
+int icnn_tc_last_launch(int32_t out[5]);
 /* FP64 tensor-core throughput probe: every warp of a full-chip grid issues `iters` x 8 independent
  * mma.m8n8k4.f64 (the instruction K2's weighted-Gram sweep is built from); *flops_out (host) = FLOPs the
  * launch performs, sink (device, 1 double) keeps the result alive.  bench.py times it with CUDA events to

@@ -45,6 +45,23 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu():
         _capi.check(-1)
 
 
+def test_tc_tuning_override_validates_its_arguments():
+    """icnn_tc_set_tuning is host-side only: out-of-range knobs are refused with ICNN_E_INVALID and a message, the
+    automatic setting is accepted; no device is touched."""
+    from icnn_b200 import _capi
+    lib = _capi.lib
+    for args, word in (((3, -1, -1), b"cfg"), ((-2, -1, -1), b"cfg"), ((-1, 3, -1), b"splitk"),
+                       ((-1, 0, -1), b"splitk"), ((-1, 16, -1), b"splitk"), ((-1, -1, 0), b"ch"),
+                       ((-1, -1, 65), b"ch")):
+        assert lib.icnn_tc_set_tuning(*args) == -1, args
+        msg = lib.icnn_last_error()
+        assert b"invalid argument" in msg and word in msg, (args, msg)
+    assert lib.icnn_tc_set_tuning(-1, -1, -1) == 0
+    out = (C.c_int32 * 5)()
+    assert lib.icnn_tc_last_launch(out) == 0
+    assert lib.icnn_tc_last_launch(None) == -1
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_no_cpu_fallback():
     import icnn_b200

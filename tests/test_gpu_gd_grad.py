@@ -56,7 +56,7 @@ def _dims_case(m, n, hidden, B, seed):
 
 @pytest.mark.parametrize("dims,B,nIter,lr,mom", [
     ((1836, 159, [600, 159]), 512, 30, 0.01, 0.3),     # C3 dims, the multi-label script's defaults
-    ((64, 512, [1024, 1024]), 200, 6, 0.01, 0.9),      # wide layers: split-K clusters in every GEMM
+    ((64, 512, [1024, 1024]), 200, 6, 0.01, 0.9),      # wide layers, K up to 1024 per GEMM
     ((12, 37, [50, 21, 33]), 77, 10, 0.02, 0.5),       # odd widths, three hidden layers, ragged tiles
 ])
 def test_matches_oracle(dims, B, nIter, lr, mom):

@@ -14,7 +14,7 @@ def gemm(A, B):
     M, K = A.shape
     N = B.shape[0]
     Cc = torch.empty(M, N, device=dev)
-    scratch = torch.empty(2 * M * K + 2 * N * K, device=dev)
+    scratch = torch.empty((2 * M + 2 * N) * ((K + 3) & ~3), device=dev)   # split operands, rows padded to 4 floats
     Ac, Bc = A.contiguous(), B.contiguous()      # keep the copies alive across the launch
     _capi.check(_capi.lib.icnn_tc_gemm_selftest(Ac.data_ptr(), Bc.data_ptr(), Cc.data_ptr(), M, N, K,
                                                 scratch.data_ptr(), stream))

@@ -14,7 +14,7 @@ for (M, N, K) in shapes:
     A = torch.randn(M, K, device=dev)
     B = torch.randn(N, K, device=dev)
     Cc = torch.full((M, N), float("nan"), device=dev)
-    scratch = torch.empty(2 * M * K + 2 * N * K, device=dev)
+    scratch = torch.empty((2 * M + 2 * N) * ((K + 3) & ~3), device=dev)   # split operands, rows padded to 4 floats
     _capi.check(_capi.lib.icnn_tc_gemm_selftest(A.data_ptr(), B.data_ptr(), Cc.data_ptr(), M, N, K, scratch.data_ptr(), stream))
     torch.cuda.synchronize()
     ref = A.double() @ B.double().T
