@@ -6,6 +6,7 @@ Public surface (mirrors the reference's, see INTEGRATION.md):
     icnn_b200.gd.solve(...)              -> unrolled momentum gradient descent
     icnn_b200.argmin_grad.argmin_grad(state, trueY, loss) -> crossEntrGrad / mseGrad + train_step_fd feeds
     icnn_b200.gd_grad.gd_grad(fg, y0, trueY, ...) -> d mse / d theta through the unrolled GD loop
+    icnn_b200.bundle_grad.bundle_grad(fg, state, trueY, loss) -> the bundle-entropy training gradient dF/dtheta
 The compute path is hand-written sm_90a CUDA behind a C ABI (libicnn_b200.so).  Every attribute above
 loads the native library on first use and raises ImportError when it is missing -- there is no CPU
 fallback.  Only ``icnn_b200.workloads`` (pure-numpy synthetic inputs, shared with the CPU reference arm of
@@ -16,11 +17,12 @@ import importlib
 _LAZY = {
     "PICNN": ("picnn", "PICNN"), "BoundPICNN": ("picnn", "BoundPICNN"),
     "bundle_entropy": ("bundle_entropy", None), "gd": ("gd", None), "argmin_grad": ("argmin_grad", None),
-    "adam": ("adam", None), "gd_grad": ("gd_grad", None), "dist": ("dist", None), "_capi": ("_capi", None),
+    "adam": ("adam", None), "gd_grad": ("gd_grad", None),
+    "bundle_grad": ("bundle_grad", None), "dist": ("dist", None), "_capi": ("_capi", None),
     "workloads": ("workloads", None),
 }
 
-__all__ = ["PICNN", "BoundPICNN", "bundle_entropy", "gd", "argmin_grad", "adam", "gd_grad"]
+__all__ = ["PICNN", "BoundPICNN", "bundle_entropy", "gd", "argmin_grad", "adam", "gd_grad", "bundle_grad"]
 
 
 def __getattr__(name):

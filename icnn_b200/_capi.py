@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 NSTAT = 8
 
 # status / enum mirrors of include/icnn_b200.h
@@ -32,6 +32,7 @@ SYMBOLS = [
     "icnn_gd_backward_workspace_bytes", "icnn_gd_backward", "icnn_fp64_mma_probe",
     "icnn_loop_graph_create", "icnn_loop_graph_launch", "icnn_loop_graph_nodes", "icnn_loop_graph_destroy",
     "icnn_tc_set_tuning", "icnn_tc_last_launch",
+    "icnn_train_grad_workspace_bytes", "icnn_train_grad",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -65,6 +66,10 @@ class BundleCfg(C.Structure):
 
 class GdGrads(C.Structure):
     _fields_ = [("dWy", _fpp), ("dWz", _fpp), ("dcy", _fpp), ("dcz", _fpp)]
+
+
+class TrainGrads(C.Structure):
+    _fields_ = [("dWy", _fpp), ("dWz", _fpp), ("dcy", _fpp), ("dcz", _fpp), ("dd", _fpp)]
 
 
 class IcnnError(RuntimeError):
@@ -113,6 +118,10 @@ def _load():
     lib.icnn_gd_backward_workspace_bytes.restype = C.c_size_t
     lib.icnn_gd_backward.argtypes = [C.c_void_p, C.POINTER(Gates), C.c_void_p, C.c_void_p, C.c_float, C.c_int32,
                                      C.c_float, C.c_float, C.c_void_p, C.POINTER(GdGrads), C.c_void_p, C.c_void_p]
+    lib.icnn_train_grad_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int64]
+    lib.icnn_train_grad_workspace_bytes.restype = C.c_size_t
+    lib.icnn_train_grad.argtypes = [C.c_void_p, C.POINTER(Gates), C.POINTER(C.c_int64), C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.POINTER(TrainGrads), C.c_void_p, C.c_void_p]
     lib.icnn_fp64_mma_probe.argtypes = [C.c_int32, C.c_void_p, C.POINTER(C.c_double), C.c_void_p]
     lib.icnn_loop_graph_create.argtypes = [C.c_void_p, C.POINTER(Gates), C.POINTER(BundleCfg), C.POINTER(BundleBufs),
                                            C.c_void_p, C.POINTER(C.c_void_p)]

@@ -29,6 +29,7 @@
 // wgrad_gemm_kernel: FP32 FFMA, reduction over the batch split over a thread-block cluster and
 // summed through distributed shared memory -- no atomics, deterministic.
 #include "gated_gemm.cuh"
+#include "gdb.cuh"
 
 #include <cstdlib>
 #include <vector>
@@ -52,13 +53,34 @@ struct WgradArgs {
   const float* A; const float* G; int lda;   // A (optionally gated by G) [Kb, lda]
   const float* D; int ldd;            // D [Kb, ldd]; nullptr = a column of ones (N == 1)
   float* C; int ldc; float kappa;     // C += kappa * (A o G)^T D
+  double* C64;                        // optional: float64 accumulation, C64 += kappa * (A o G)^T D (C unused)
 };
 
 // C[m, n] += kappa * sum_b A[b, m] G[b, m] D[b, n].  64x64 tile, 16 batch rows per stage; both
 // operands are read along their contiguous dimension.  gridDim.z = S CTAs of one cluster split the
 // batch and reduce their partial tiles through DSMEM (same scheme as gated_gemm_kernel).
+// Acc = double (WgradArgs::C64): every product of two floats is exact in float64 and the sums over the batch and
+// the split are float64, so the result does not depend on how the rows are split over launches (train_grad.cu).
+constexpr int WG_TILE_BYTES = (int)sizeof(float) * (2 * BK * (BM + PAD) + 2 * BK * (BN + PAD));
+template <typename Acc>
+struct WgSmem {
+  static constexpr int PART = (int)sizeof(Acc) * BM * (BN + 1);
+  static constexpr int BYTES = PART > WG_TILE_BYTES ? PART : WG_TILE_BYTES;
+};
+__device__ __forceinline__ float wg_madd(float x, float y, float acc) { return fmaf(x, y, acc); }
+__device__ __forceinline__ double wg_madd(float x, float y, double acc) { return fma((double)x, (double)y, acc); }
+__device__ __forceinline__ void wg_store(const WgradArgs& a, int m, int nn, float v) {
+  float* c = a.C + (long long)m * a.ldc + nn;
+  *c = fmaf(a.kappa, v, *c);
+}
+__device__ __forceinline__ void wg_store(const WgradArgs& a, int m, int nn, double v) {
+  a.C64[(long long)m * a.ldc + nn] += (double)a.kappa * v;
+}
+
+template <typename Acc>
 __global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
-  __shared__ __align__(16) float smem_f[2 * BK * (BM + PAD) + 2 * BK * (BN + PAD)];
+  __shared__ __align__(16) unsigned char smem_raw[WgSmem<Acc>::BYTES];
+  float* smem_f = reinterpret_cast<float*>(smem_raw);
   float (*As)[BK][BM + PAD] = reinterpret_cast<float (*)[BK][BM + PAD]>(smem_f);
   float (*Bs)[BK][BN + PAD] = reinterpret_cast<float (*)[BK][BN + PAD]>(smem_f + 2 * BK * (BM + PAD));
   const int t = threadIdx.x;
@@ -89,11 +111,11 @@ __global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
     for (int i = 0; i < 4; ++i) { As[buf][l_k][l_c + i] = ra[i]; Bs[buf][l_k][l_c + i] = rb[i]; }
   };
 
-  float acc[4][4];
+  Acc acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int j = 0; j < 4; ++j) acc[i][j] = Acc(0);
 
   const int nk_all = (a.Kb + BK - 1) / BK;
   const int kt0 = (int)(((long long)nk_all * blockIdx.z) / S);
@@ -112,7 +134,7 @@ __global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
+        for (int j = 0; j < 4; ++j) acc[i][j] = wg_madd(aa[i], bb[j], acc[i][j]);
     }
     if (kt + 1 < nk) store_tiles(buf ^ 1);
     __syncthreads();
@@ -126,16 +148,13 @@ __global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int nn = n0 + tx * 4 + j;
-        if (nn < a.N) {
-          float* c = a.C + (long long)m * a.ldc + nn;
-          *c = fmaf(a.kappa, acc[i][j], *c);
-        }
+        if (nn < a.N) wg_store(a, m, nn, acc[i][j]);
       }
     }
     return;
   }
   cg::cluster_group cluster = cg::this_cluster();
-  float (*Ps)[BN + 1] = reinterpret_cast<float (*)[BN + 1]>(smem_f);
+  Acc (*Ps)[BN + 1] = reinterpret_cast<Acc (*)[BN + 1]>(smem_raw);
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -145,13 +164,10 @@ __global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
   const int r_lo = (BM * rank) / S, r_hi = (BM * (rank + 1)) / S;
   for (int idx = t; idx < (r_hi - r_lo) * BN; idx += 256) {
     const int rr = r_lo + idx / BN, cc = idx % BN;
-    float v = 0.f;
+    Acc v = Acc(0);
     for (int q = 0; q < S; ++q) v += *cluster.map_shared_rank(&Ps[rr][cc], q);
     const int m = m0 + rr, nn = n0 + cc;
-    if (m < a.M && nn < a.N) {
-      float* c = a.C + (long long)m * a.ldc + nn;
-      *c = fmaf(a.kappa, v, *c);
-    }
+    if (m < a.M && nn < a.N) wg_store(a, m, nn, v);
   }
   cluster.sync();
 }
@@ -170,7 +186,19 @@ static cudaError_t launch_wgrad(const WgradArgs& a, cudaStream_t st) {
   lattr[0].id = cudaLaunchAttributeClusterDimension;
   lattr[0].val.clusterDim.x = 1; lattr[0].val.clusterDim.y = 1; lattr[0].val.clusterDim.z = S;
   cfg.attrs = lattr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, wgrad_gemm_kernel, a);
+  if (a.C64) return cudaLaunchKernelEx(&cfg, wgrad_gemm_kernel<double>, a);
+  return cudaLaunchKernelEx(&cfg, wgrad_gemm_kernel<float>, a);
+}
+
+// dst[r, j] += c[r] * src[r, j]
+__global__ void row_axpy_kernel(float* dst, const float* src, const float* c, long long N, int w) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < N) dst[i] = fmaf(c[i / w], src[i], dst[i]);
+}
+
+void launch_row_axpy(float* dst, const float* src, const float* c, long long rows, int w, cudaStream_t st) {
+  const long long N = rows * w;
+  if (N > 0) row_axpy_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(dst, src, c, N, w);
 }
 
 // dst += kappa * src
@@ -233,18 +261,9 @@ __global__ void tangent_stage_kernel(StageArgs a) {
   else { a.dcz[idx] = acc * a.wz[j]; a.Sout[idx] = acc; }
 }
 
-struct GdbLayout {
-  size_t Z[ICNN_MAX_LAYERS], Zt[ICNN_MAX_LAYERS], Dacc[ICNN_MAX_LAYERS], dl[2], y, v, g, a, f, tc, total;
-  bool use_tc;
-  // stored-pattern mode (single pass): per-iteration stores and the phase-2 scratch
-  bool stored;
-  size_t kap, Zs[ICNN_MAX_LAYERS], Ds[ICNN_MAX_LAYERS], As[ICNN_MAX_LAYERS], Zts[ICNN_MAX_LAYERS], Ty[ICNN_MAX_LAYERS];
-  size_t P_hi, P_lo, Pk, Sout;
-};
-
 // tensor-core GEMMs (3xTF32) for the forward / tangent / backward products once a 128-row tile fills;
 // ICNN_GDB=simt keeps the FP32 FFMA kernels
-static bool gdb_use_tc(const icnn_picnn* h, int B) {
+bool gdb_use_tc(const icnn_picnn* h, int B) {
   const char* v = getenv("ICNN_GDB");
   return h->use_tc && B >= 64 && !(v && v[0] == 's');
 }
@@ -260,7 +279,7 @@ static bool gdb_want_stored(const icnn_picnn* h, int B, int nIter, size_t store_
   return (double)store_floats * 4.0 <= cap * 1073741824.0;
 }
 
-static GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
+GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
   GdbLayout lo{};
   size_t off = 0;
   auto take = [&](size_t nfl) { size_t o = off; off += (nfl + 63) & ~(size_t)63; return o; };
@@ -306,11 +325,9 @@ static GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
 // One GD iteration's primal forward + backward.  acc != nullptr: also the tangent forward and the
 // gradient accumulations (pass 2 of the two-pass mode).  store_it >= 0 (stored-pattern mode, tensor-core
 // path only): the primal pass writes Z_l, delta_l and delta_l Wz_l^T of this iteration into the stores
-// and accumulates Delta_l += kappa delta_l.
-struct GdbAcc { const icnn_gd_grads* gr; float kappa; };
-
-static int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo,
-                         const GdbAcc* acc, int store_it, float store_kappa, cudaStream_t st) {
+// and accumulates Delta_l += kappa delta_l.  (GdbAcc: gdb.cuh)
+int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo,
+                  const GdbAcc* acc, int store_it, float store_kappa, cudaStream_t st) {
   const int B = gt->B, n = h->n, L = h->L;
   float* y = ws + lo.y; float* g = ws + lo.g; float* f = ws + lo.f; float* av = ws + lo.a;
   float* dl[2] = {ws + lo.dl[0], ws + lo.dl[1]};
@@ -348,6 +365,8 @@ static int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, c
       GDB_LAUNCH(launch_gemm<2>(a, st), "gd_backward tangent");
     }
   }
+  if (acc && acc->c)   // train_grad: the backward accumulates with c o Z_l + Zt_l in place of the tangent
+    for (int i = 0; i < L; ++i) launch_row_axpy(ws + lo.Zt[i], ws + lo.Z[i], acc->c, B, h->hidden[i], st);
   const int sl = h->hidden[L - 1];
   const long long NL = (long long)B * sl;
   float* dlast = store_it >= 0 ? tb.dstore[L - 1] : dl[0];     // plain delta_{L-1}
@@ -361,7 +380,7 @@ static int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, c
                                                                       h->Wcat[L], kp, NL, sl);
     WgradArgs w{};   // dWz_L [s_{L-1}, 1] += kappa * sum_b zt_{L-1} o cz_L   (delta_L = 1)
     w.M = sl; w.N = 1; w.Kb = B; w.A = ws + lo.Zt[L - 1]; w.G = gt->cz[L]; w.lda = sl; w.D = nullptr; w.ldd = 1;
-    w.C = acc->gr->dWz[L]; w.ldc = 1; w.kappa = kp;
+    w.C = acc->gr->dWz[L]; w.ldc = 1; w.kappa = kp; w.C64 = acc->w64 ? acc->w64->dWz[L] : nullptr;
     GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(L)");
   }
   int cur = 0;
@@ -370,6 +389,7 @@ static int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, c
       WgradArgs w{};
       w.M = h->prev(i); w.N = h->hidden[i]; w.Kb = B; w.A = ws + lo.Zt[i - 1]; w.G = gt->cz[i]; w.lda = w.M;
       w.D = dl[cur]; w.ldd = w.N; w.C = acc->gr->dWz[i]; w.ldc = w.N; w.kappa = acc->kappa;
+      w.C64 = acc->w64 ? acc->w64->dWz[i] : nullptr;
       GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad");
     }
     if (lo.use_tc) {
@@ -389,6 +409,32 @@ static int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, c
     GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward backward");
     cur ^= 1;
   }
+  return ICNN_OK;
+}
+
+int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo, const float* av,
+                    const icnn_gd_grads* gr, float ksum, const GdbW64* w64, cudaStream_t st) {
+  const int B = gt->B, n = h->n, L = h->L;
+  const long long N = (long long)B * n;
+  for (int l = 0; l < L; ++l) {
+    WgradArgs w{};
+    w.M = n; w.N = h->hidden[l]; w.Kb = B; w.A = av; w.G = gt->cy[l]; w.lda = n;
+    w.D = ws + lo.Dacc[l]; w.ldd = w.N; w.C = gr->dWy[l]; w.ldc = w.N; w.kappa = 1.f;
+    w.C64 = w64 ? w64->dWy[l] : nullptr;
+    GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy)");
+    GemmArgs a{};   // dcy_l = a o (Delta_l Wy_l^T): the backward GEMM against the Wy rows of Wcat_l
+    a.M = B; a.N0 = 0; a.N = n; a.K0 = h->hidden[l]; a.K1 = 0; a.A0 = ws + lo.Dacc[l]; a.lda0 = a.K0;
+    a.W = h->Wcat[l] + (size_t)h->prev(l) * h->hidden[l]; a.ldw = a.K0; a.alpha = h->alpha;
+    a.Cy = av; a.g = gr->dcy[l]; a.g_row_stride = n; a.n = n; a.g_scale = 1.f;
+    GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward dcy");
+  }
+  // output layer: Delta_L = ksum for every row
+  WgradArgs w{};
+  w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gt->cy[L]; w.lda = n; w.D = nullptr; w.ldd = 1;
+  w.C = gr->dWy[L]; w.ldc = 1; w.kappa = ksum; w.C64 = w64 ? w64->dWy[L] : nullptr;
+  GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
+  rowbcast_fma_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], ksum,
+                                                                  N, n);
   return ICNN_OK;
 }
 
@@ -496,7 +542,7 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
     ICNN_CUDA_CHECK(cudaMemcpyAsync(ws + lo.y, y0, sizeof(float) * N, cudaMemcpyDeviceToDevice, st));
     ICNN_CUDA_CHECK(cudaMemsetAsync(ws + lo.v, 0, sizeof(float) * N, st));
     for (int it = 0; it < nIter; ++it) {
-      GdbAcc acc{gr, kappa[it]};
+      GdbAcc acc{gr, kappa[it], nullptr, nullptr};
       int rc = gdb_iteration(h, gates, ws, lo, pass ? &acc : nullptr, -1, 0.f, st);
       if (rc) return rc;
       gd_update_kernel<<<gN, 256, 0, st>>>(ws + lo.y, ws + lo.v, ws + lo.g, N, lr, momentum);
@@ -512,24 +558,9 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
     }
   }
 
-  // y-gate terms from the accumulated Delta_l
-  for (int l = 0; l < L && nIter > 0; ++l) {
-    WgradArgs w{};
-    w.M = n; w.N = h->hidden[l]; w.Kb = B; w.A = av; w.G = gates->cy[l]; w.lda = n;
-    w.D = ws + lo.Dacc[l]; w.ldd = w.N; w.C = gr->dWy[l]; w.ldc = w.N; w.kappa = 1.f;
-    GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy)");
-    GemmArgs a{};   // dcy_l = a o (Delta_l Wy_l^T): the backward GEMM against the Wy rows of Wcat_l
-    a.M = B; a.N0 = 0; a.N = n; a.K0 = h->hidden[l]; a.K1 = 0; a.A0 = ws + lo.Dacc[l]; a.lda0 = a.K0;
-    a.W = h->Wcat[l] + (size_t)h->prev(l) * h->hidden[l]; a.ldw = a.K0; a.alpha = h->alpha;
-    a.Cy = av; a.g = gr->dcy[l]; a.g_row_stride = n; a.n = n; a.g_scale = 1.f;
-    GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward dcy");
-  }
-  if (nIter > 0) {   // output layer: Delta_L = sum_i kappa_i for every sample
-    WgradArgs w{};
-    w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gates->cy[L]; w.lda = n; w.D = nullptr; w.ldd = 1;
-    w.C = gr->dWy[L]; w.ldc = 1; w.kappa = (float)ksum;
-    GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
-    rowbcast_fma_kernel<<<gN, 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], (float)ksum, N, n);
+  if (nIter > 0) {
+    int rc = gdb_ygate_stage(h, gates, ws, lo, av, gr, (float)ksum, nullptr, st);
+    if (rc) return rc;
   }
   ICNN_CUDA_CHECK(cudaGetLastError());
   return ICNN_OK;

@@ -73,9 +73,11 @@ def gd_grad(fg: BoundPICNN, y0, trueY, nIter=30, lr=0.01, momentum=0.3, loss_sca
     return host(yN), {k: [host(t) for t in v] for k, v in grads.items()}
 
 
-def _xpath_backward(net, x, dcy, dcz):
+def _xpath_backward(net, x, dcy, dcz, dd=None):
     """Dense-layer backprop of the gate adjoints into the x-path parameters
-    (multi-label-cls/icnn-back.py:255-262 u path, :269-272 cz gate, :279-281 cy gate)."""
+    (multi-label-cls/icnn-back.py:255-262 u path, :269-272 cz gate, :279-281 cy gate).  ``dd`` (the adjoints of
+    the additive gates d_l = P_l Wzx_l + bzx_l, multi-label-cls/icnn_ebundle.py:372-373) adds 'Wzx' / 'bzx'; the GD-mode energy gradient has
+    none, so by default they are left out."""
     L = net.L
     us, pres, p = [], [], x
     for i in range(L):
@@ -84,12 +86,18 @@ def _xpath_backward(net, x, dcy, dcz):
         pres.append(pre); us.append(u); p = u
     out = dict(Wu=[None] * L, bu=[None] * L, Wzu=[None] * (L + 1), bzu=[None] * (L + 1),
                Wyu=[None] * (L + 1), byu=[None] * (L + 1))
+    if dd is not None:
+        out.update(Wzx=[None] * (L + 1), bzx=[None] * (L + 1))
     dU = [torch.zeros_like(u) for u in us]
     for i in range(L, -1, -1):
         P = x if i == 0 else us[i - 1]
         out["Wyu"][i] = P.t() @ dcy[i]
         out["byu"][i] = dcy[i].sum(0)
         dP = dcy[i] @ net.Wyu[i].t()
+        if dd is not None:
+            out["Wzx"][i] = P.t() @ dd[i]
+            out["bzx"][i] = dd[i].sum(0)
+            dP = dP + dd[i] @ net.Wzx[i].t()
         if i > 0:
             pz = dcz[i] * (torch.addmm(net.bzu[i], P, net.Wzu[i]) > 0)
             out["Wzu"][i] = P.t() @ pz

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ICNN_ABI_VERSION 4
+#define ICNN_ABI_VERSION 5
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -231,6 +231,31 @@ size_t icnn_gd_backward_workspace_bytes(const icnn_picnn_t* h, int32_t B, int32_
 int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, const float* y0, const float* trueY,
                      float loss_scale, int32_t nIter, float lr, float momentum, float* yN,
                      const icnn_gd_grads* grads, void* workspace, void* stream);
+
+/* ---- bundle-entropy training gradient (SURVEY.md section 8f, row 1: the step after K3) ---------------- */
+/* replaces: opt.compute_gradients(F_, theta_) (multi-label-cls/icnn_ebundle.py:154) on the surrogate
+ *   F_ = c * E(x, y) + sum_j v_j dE/dy_j          (multi-label-cls/icnn_ebundle.py:148)
+ * fed the train_step_fd rows (:296-314) in CSR form: sample u owns rows row_offsets[u] .. row_offsets[u+1]
+ * (host int64 [B+1], row_offsets[0] = 0, non-decreasing, R = row_offsets[B]) of Y [R, n] (bundle points),
+ * V [R, n] and c [R] (all device f32, the reference's float32 placeholders :129-131); row r sees the gates of
+ * its sample (the bound minibatch's row u).  Returns d (sum of F_ over all rows) / d (y-path weights and gates):
+ *   dWy[l] [n, s_l], dWz[l] [s_{l-1}, s_l]   summed over every row
+ *   dcy[l] [B, n], dcz[l] [B, s_{l-1}], dd[l] [B, s_l]   per sample (summed over the sample's rows)
+ * for l = 0..L ([0] of dWz/dcz unused).  All buffers device f32, overwritten.  The x-path parameters follow from
+ * (dcy, dcz, dd) by dense-layer backprop on the caller's side.  workspace =
+ * icnn_train_grad_workspace_bytes(h, B, R) device bytes; rows are processed in chunks, so it does not grow with R
+ * beyond ICNN_TRAIN_WS_GB (default 2) GiB.  The affine RL wrapper is not supported (ICNN_E_UNSUPPORTED): the
+ * RL code's bundle path is disabled in the reference (RL/src/icnn.py:84). */
+typedef struct {
+  float* const* dWy;
+  float* const* dWz;
+  float* const* dcy;
+  float* const* dcz;
+  float* const* dd;
+} icnn_train_grads;
+size_t icnn_train_grad_workspace_bytes(const icnn_picnn_t* h, int32_t B, int64_t R);
+int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, const int64_t* row_offsets, const float* Y,
+                    const float* V, const float* c, const icnn_train_grads* grads, void* workspace, void* stream);
 
 /* ---- RL Adam argmin (SURVEY.md section 8f, row 3) -------------------------------------------------- */
 /* replaces: Agent.adam (RL/src/icnn.py:160-215) applied to [negQ - entropy(act), d/dact]
