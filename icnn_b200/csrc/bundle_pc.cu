@@ -104,6 +104,7 @@ int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int 
   a.b = *b; a.c = *cfg; a.t = t; a.npad = c.npad;
   a.flags = 0;
   if (const char* v = getenv("ICNN_PC_FLAGS")) a.flags = atoi(v);
+  if (const char* v = getenv("ICNN_PC_LEGACY")) { if (v[0] == '1') a.flags |= 4; }
   cudaError_t e;
   const int key = (c.v3 ? 3000 : 0) + (c.gv ? 2000 : 0) + (c.vec ? 0 : 1000) + c.wps * 10 + c.nch;
   switch (key) {

@@ -17,6 +17,12 @@
 //   u = G^T z is maintained incrementally (u += alpha (v1 + sigma v2 + v3)), so ry = logit(y) + u costs one
 //       log per element per iteration and no pass.
 //
+// Passes over a sample's k bundle rows per outer iteration (at n_y = 4096 a row is 16 KB and the rows of the resident
+// samples do not fit in L2, so each pass is mostly HBM traffic):
+//   append (Gram row + duplicate flags) 1; dependency test 1 residual pass, + 1 dot pass and 1 more residual pass when
+//   it refines; u0 = G^T z0 1; per interior-point iteration: sweep A 1 (rb = ceil((k + 2) / 8) <= 4; V3 also rb = 5,
+//   see gram_pass_pc) and sweep B 1.  ~8 interior-point iterations at C5 -> about 2 its + 3 passes.
+//
 // Shared memory per sample: 4 n-vectors (y, u, ry|du, v1+v3|dy), ONE packed lower-triangular k x k matrix,
 // 18 k-vectors.  All reductions over n_y and all k x k algebra are FP64, as in the reference.
 //
@@ -37,7 +43,8 @@ struct PcArgs {
   icnn_bundle_cfg c;
   int t;
   int npad;  // doubles reserved per n-vector
-  int flags; // exploration knobs (bundle_pc.cu): bit 0 = general k x k stage even for k <= 32, bit 1 = plain stores for xs
+  int flags; // exploration knobs (bundle_pc.cu): bit 0 = general k x k stage even for k <= 32, bit 1 = plain stores for xs,
+             // bit 2 = sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY)
 };
 
 constexpr int PC_NKV = 18;
@@ -367,14 +374,22 @@ __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const
 }
 
 // k + 2 sweep rows in rb = ceil((k + 2) / 8) <= 8 row blocks (k <= 62).  On return warp 0 has stored M0, q, w.
-template <int WPS, bool VEC, bool GVL, class G>
+// rb <= 4 (and rb = 5 with ONE5): one sweep, every row block loaded once.  Larger rb: the upper triangle of blocks 0-3,
+// then that of blocks 4.., then blocks 0-1 and 2-3 against blocks 4.. (8 + 3 (rb - 4) block loads; 21+ tiles of
+// accumulators in one sweep would spill).  ONE5 (V3 build only: the other builds have no register room for 15 tiles)
+// enables the one-sweep rb = 5, which at C5 carries the last outer iterations (k = 31..38); split5 sends rb = 5 through
+// the composition anyway (11 block loads instead of 5; ICNN_PC_LEGACY=1, the form the one sweep is tested against).
+template <int WPS, bool VEC, bool GVL, bool ONE5, class G>
 __device__ __forceinline__ void gram_pass_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
-                                             const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap) {
+                                             const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
+                                             bool split5) {
   const int rb = (k + 2 + 7) >> 3;
   if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
   else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
   else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
-  else {
+  else if (ONE5 && rb == 5 && !split5) {
+    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
+  } else {
     gram_sweep_pc<WPS, 4, 4, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
     if (rb > 4) {
       const int r2 = rb - 4;
@@ -391,7 +406,8 @@ __device__ __forceinline__ void gram_pass_pc(const G& g, const float* const* row
 template <int T, bool VEC>
 __device__ __forceinline__ int pc_col(int cb, int tid, int c) { return VEC ? cb + 4 * tid + c : cb + tid + c * T; }
 
-template <int T, int NR, bool VEC>
+// UNR: rows per unrolled trip of the row loop = row loads in flight per thread (the pass is bound by them)
+template <int T, int NR, bool VEC, int UNR = 4>
 __device__ __forceinline__ void col_dots_pc(const float* const* rowp, int k, int n, int cb, int tid,
                                             const double* const (&w)[NR], double (&acc)[NR][4]) {
 #pragma unroll
@@ -400,7 +416,7 @@ __device__ __forceinline__ void col_dots_pc(const float* const* rowp, int k, int
     for (int c = 0; c < 4; ++c) acc[q][c] = 0.0;
   const bool in0 = VEC ? (cb + 4 * tid < n) : (cb + tid < n);
   const bool full = VEC ? in0 : (cb + tid + 3 * T < n);
-#pragma unroll 4
+#pragma unroll UNR
   for (int j = 0; j < k; ++j) {
     const float* p = rowp[j];
     float v[4] = {0.f, 0.f, 0.f, 0.f};
@@ -700,7 +716,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     double* zc = PCKV(1 + zsel);
     double* scur = PCKV(3 + zsel);
     // ---- sweep A (warp 0 ends up holding M0, q, w in shared memory)
-    gram_pass_pc<WPS, VEC, GV>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad);
+    gram_pass_pc<WPS, VEC, GV, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, (A.flags & 4) != 0);
     // ---- k x k stage
     if (g.warp == 0) {
       const PcKxk io{Lp, invd, zc, scur, wk, hk, qk, dza, dzp, dzq, dsa, sc, isc};
@@ -721,7 +737,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
         const int cb = ch * 4 * T;
         if (cb >= n) break;
         double acc[3][4];
-        col_dots_pc<T, 3, VEC>(rowp, k, n, cb, g.tid, w3, acc);
+        col_dots_pc<T, 3, VEC, V3 ? 8 : 4>(rowp, k, n, cb, g.tid, w3, acc);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const int e = pc_col<T, VEC>(cb, g.tid, c);
