@@ -3,6 +3,7 @@
 Public surface (mirrors the reference's, see INTEGRATION.md):
     icnn_b200.bundle_entropy.solveBatch(fg, initXs, nIter, callback, solver, variant=...)
     icnn_b200.PICNN(...).bind(x)         -> the fg object for the fused on-device loop
+    icnn_b200.ConvPICNN.from_variables(vars, H, W).bind(x) -> the same for the image-completion conv PICNN
     icnn_b200.gd.solve(...)              -> unrolled momentum gradient descent
     icnn_b200.argmin_grad.argmin_grad(state, trueY, loss) -> crossEntrGrad / mseGrad + train_step_fd feeds
     icnn_b200.gd_grad.gd_grad(fg, y0, trueY, ...) -> d mse / d theta through the unrolled GD loop
@@ -16,13 +17,15 @@ import importlib
 
 _LAZY = {
     "PICNN": ("picnn", "PICNN"), "BoundPICNN": ("picnn", "BoundPICNN"),
+    "ConvPICNN": ("conv_picnn", "ConvPICNN"), "BoundConvPICNN": ("conv_picnn", "BoundConvPICNN"),
+    "conv_picnn": ("conv_picnn", None),
     "bundle_entropy": ("bundle_entropy", None), "gd": ("gd", None), "argmin_grad": ("argmin_grad", None),
     "adam": ("adam", None), "gd_grad": ("gd_grad", None),
     "bundle_grad": ("bundle_grad", None), "dist": ("dist", None), "_capi": ("_capi", None),
     "workloads": ("workloads", None),
 }
 
-__all__ = ["PICNN", "BoundPICNN", "bundle_entropy", "gd", "argmin_grad", "adam", "gd_grad", "bundle_grad"]
+__all__ = ["PICNN", "BoundPICNN", "ConvPICNN", "BoundConvPICNN", "conv_picnn", "bundle_entropy", "gd", "argmin_grad", "adam", "gd_grad", "bundle_grad"]
 
 
 def __getattr__(name):

@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 NSTAT = 8
 
 # status / enum mirrors of include/icnn_b200.h
@@ -33,6 +33,8 @@ SYMBOLS = [
     "icnn_loop_graph_create", "icnn_loop_graph_launch", "icnn_loop_graph_nodes", "icnn_loop_graph_destroy",
     "icnn_tc_set_tuning", "icnn_tc_last_launch",
     "icnn_train_grad_workspace_bytes", "icnn_train_grad",
+    "icnn_conv_picnn_create", "icnn_conv_picnn_destroy", "icnn_conv_picnn_workspace_bytes", "icnn_conv_picnn_fg",
+    "icnn_conv_solve_batch_fused", "icnn_conv_gd_solve",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -41,6 +43,12 @@ _fpp = C.POINTER(C.c_void_p)
 class PicnnDesc(C.Structure):
     _fields_ = [("n", C.c_int32), ("L", C.c_int32), ("hidden", C.POINTER(C.c_int32)),
                 ("alpha", C.c_float), ("Wy", _fpp), ("Wz", _fpp)]
+
+
+class ConvPicnnDesc(C.Structure):
+    _fields_ = [("H", C.c_int32), ("W", C.c_int32), ("Lc", C.c_int32), ("C", C.POINTER(C.c_int32)),
+                ("k", C.POINTER(C.c_int32)), ("s", C.POINTER(C.c_int32)), ("Ld", C.c_int32),
+                ("fcs", C.POINTER(C.c_int32)), ("Wz", _fpp), ("Wy", _fpp), ("Wred", _fpp), ("bred", _fpp)]
 
 
 class Gates(C.Structure):
@@ -129,6 +137,13 @@ def _load():
     lib.icnn_loop_graph_nodes.argtypes = [C.c_void_p]
     lib.icnn_loop_graph_nodes.restype = C.c_int64
     lib.icnn_loop_graph_destroy.argtypes = [C.c_void_p]
+    lib.icnn_conv_picnn_create.argtypes = [C.POINTER(ConvPicnnDesc), C.POINTER(C.c_void_p), C.c_void_p]
+    lib.icnn_conv_picnn_destroy.argtypes = [C.c_void_p]
+    lib.icnn_conv_picnn_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    lib.icnn_conv_picnn_workspace_bytes.restype = C.c_size_t
+    lib.icnn_conv_picnn_fg.argtypes = lib.icnn_picnn_fg.argtypes
+    lib.icnn_conv_solve_batch_fused.argtypes = lib.icnn_solve_batch_fused.argtypes
+    lib.icnn_conv_gd_solve.argtypes = lib.icnn_gd_solve.argtypes
     for name in SYMBOLS:
         getattr(lib, name)  # AttributeError if the .so does not export it
     if lib.icnn_abi_version() != ABI_VERSION:

@@ -8,8 +8,9 @@ returning ``(x, A, b, lam, xs, nIters)`` (callers name A, b as G, h:
 multi-label-cls/icnn_ebundle.py:225).
 
 Two ways to supply ``fg``:
-  * fused mode   -- ``fg`` is a :class:`icnn_b200.BoundPICNN` (``PICNN.bind(x)``): the whole loop
-                    (K1 PICNN f/grad kernel + K2 bundle step) runs on the device, no host round
+  * fused mode   -- ``fg`` is a :class:`icnn_b200.BoundPICNN` (``PICNN.bind(x)``) or a
+                    :class:`icnn_b200.BoundConvPICNN` (``ConvPICNN.bind(x)``): the whole loop
+                    (f/grad kernels + K2 bundle step) runs on the device, no host round
                     trip per iteration;
   * callback mode -- ``fg`` is any Python callable ``fg(x ndarray[B,n]) -> (f[B], g[B,n])``
                     (e.g. a conv-PICNN in torch): one host hop per iteration like the reference,
@@ -25,6 +26,7 @@ import numpy as np
 import torch
 
 from . import _capi
+from .conv_picnn import BoundConvPICNN
 from .picnn import BoundPICNN, default_device
 
 __all__ = ["solveBatch", "solve", "BundleState", "VARIANT_DEFAULTS"]
@@ -279,7 +281,10 @@ def solveBatch(fg, initXs, nIter=None, callback=None, solver="pc", *, variant="l
     nIter = int(nIter)
     if not torch.cuda.is_available():
         raise RuntimeError("icnn_b200.solveBatch needs a CUDA device (no CPU fallback)")
-    fused = isinstance(fg, BoundPICNN)
+    conv = isinstance(fg, BoundConvPICNN)
+    fused = conv or isinstance(fg, BoundPICNN)
+    if conv and graph:
+        raise ValueError("solveBatch: graph=True is not supported with a conv PICNN fg")
     dev = fg.net.device if fused else (torch.device(device) if device is not None else default_device())
     x0 = initXs
     B, n = x0.shape
@@ -324,13 +329,15 @@ def solveBatch(fg, initXs, nIter=None, callback=None, solver="pc", *, variant="l
             if graph:
                 _capi.check(_capi.lib.icnn_loop_graph_launch(st.loop_graph(fg, cfg), stream))
             else:
-                _capi.check(_capi.lib.icnn_solve_batch_fused(fg.net._h, C.byref(fg.c_gates), C.byref(cfg),
-                                                             C.byref(st.c), fg.ws.data_ptr(), stream))
+                solve = _capi.lib.icnn_conv_solve_batch_fused if conv else _capi.lib.icnn_solve_batch_fused
+                _capi.check(solve(fg.net._h, C.byref(fg.c_gates), C.byref(cfg), C.byref(st.c), fg.ws.data_ptr(),
+                                  stream))
         else:
             _capi.check(_capi.lib.icnn_bundle_init(C.byref(st.c), nIter, stream))
             for t in range(nIter):
                 if fused:
-                    _capi.check(_capi.lib.icnn_picnn_fg(
+                    fg_fn = _capi.lib.icnn_conv_picnn_fg if conv else _capi.lib.icnn_picnn_fg
+                    _capi.check(fg_fn(
                         fg.net._h, C.byref(fg.c_gates), st.y32.data_ptr(), st.f.data_ptr(),
                         st.G.data_ptr(), 0, st.perm.data_ptr(), st.count.data_ptr(), KS,
                         fg.ws.data_ptr(), None, stream))

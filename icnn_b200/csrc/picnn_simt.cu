@@ -118,6 +118,11 @@ void out_layer_launch(const icnn_picnn* h, const icnn_gates* gt, const float* Zl
   else out_layer_kernel<32><<<cdiv(B * 32, 256), 256, 0, st>>>(o);
 }
 
+// host launcher of gd_update_kernel for the other translation units (conv_picnn.cu; declared in tc_gemm.cuh)
+void gd_update_launch(float* y, float* v, const float* g, long long N, float lr, float mom, cudaStream_t st) {
+  gd_update_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(y, v, g, N, lr, mom);
+}
+
 bool picnn_tc_supported(const icnn_picnn* h);
 int picnn_tc_prepare_weights(icnn_picnn* h, cudaStream_t st);
 void picnn_tc_free_weights(icnn_picnn* h);

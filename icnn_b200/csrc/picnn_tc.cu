@@ -18,7 +18,7 @@
 //               afterwards every warp runs the fused epilogue on the 16 rows its accumulators hold
 //   warp 8      TMA producer: cp.async.bulk.tensor.2d of A_hi/A_lo/B_hi/B_lo boxes (32 fp32 = 128 B
 //               wide) into an NST-stage ring, mbarrier expect_tx
-#include "common.cuh"
+#include "tc_gemm.cuh"
 
 #include <cuda.h>
 #include <cooperative_groups.h>
@@ -157,31 +157,7 @@ constexpr int TC_CH = 1;   // default half k-blocks per accumulation chunk (K = 
 constexpr int TC_CONSUMER_WARPS = 8;
 constexpr int TC_THREADS = 32 * (TC_CONSUMER_WARPS + 1);
 
-struct TcArgs {
-  int M, N, K;
-  int ch;    // half k-blocks per accumulation chunk (>= 1), set by launch_tc_gemm
-  int mode;  // 0 forward, 1 backward, 2 plain store (self test)
-  // forward epilogue: Z = act(acc + D); optional next-layer operand A'_{next}[:, 0:N] = Z o Cz_next (hi/lo)
-  const float* D; float* Z; float alpha;
-  const float* Cz_next; float* nxt_hi; float* nxt_lo; int nxt_ld;
-  // backward epilogue: columns < N0 -> delta_prev = act'(Zprev) o Cz o acc (hi/lo, row pitch dprev_ld); else g += ...
-  int N0; const float* Zprev; const float* Cz; float* dprev_hi; float* dprev_lo; int dprev_ld;
-  const float* Cy; float* g; long long g_row_stride; const int* perm; const int* count; int KS; int n;
-  float g_scale;
-  float* C;  // mode 2
-  // GD training backward (GDB instantiation only, gd_backward.cu):
-  //   mode 0 with tangent != 0: Z = act'(D) o acc (D holds the primal activation), no bias
-  //   mode 1: optional plain copy of delta_prev, dCz += kappa * Ztprev o acc, Dacc += kappa * delta_prev
-  //   mode 0 with tangent == 2 (stored-pattern phase): Z = act'(Zmask) o (acc + D[(row % drow_mod), :])
-  //   mode 1: optional plain copy of the pre-gating product acc (acc_plain, [M, N0])
-  int tangent; float* dprev_plain; float* dCz; const float* Ztprev; float* Dacc; float kappa;
-  const float* Zmask; int drow_mod; float* acc_plain;
-  // mode 3 (x-path gate GEMM): out = acc + bias[col]; up to 4 column ranges [rbeg[r], rbeg[r+1]) each with
-  // its own ReLU flag and destination (row pitch rld[r]); range 0 may instead be written as a TF32
-  // hi/lo pair (the next u-layer operand)
-  int nr; int rbeg[5]; int rrelu[4]; float* rdst[4]; int rld[4]; float* r0_hi; float* r0_lo; const float* bias;
-  const int* skip_if_zero;
-};
+// TcArgs: tc_gemm.cuh
 
 template <int BN, int NST_>
 struct TcSmem {
@@ -643,8 +619,8 @@ static std::atomic<int> g_tc_cfg{-1}, g_tc_splitk{-1}, g_tc_ch{-1};
 // {BN, NST, splitk, ch, mode} of the calling thread's most recent launch_tc_gemm (icnn_tc_last_launch)
 static thread_local int g_tc_last[5] = {0, 0, 0, 0, -1};
 
-static int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const float* Bh, const float* Bl, long long ldb,
-                          TcArgs a, cudaStream_t st, bool gdb = false) {
+int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const float* Bh, const float* Bl, long long ldb,
+                   TcArgs a, cudaStream_t st, bool gdb) {
   const int gy = cdiv(a.M, TC_BM);
   // tile choice: 64-wide tiles; two CTAs per SM (the epilogue of one overlaps the main loop of the
   // other) once there are >= 2 tiles per SM, else one CTA per SM with a 4-deep ring.

@@ -14,13 +14,17 @@ import numpy as np
 import torch
 
 from . import _capi
+from .conv_picnn import BoundConvPICNN
 from .picnn import BoundPICNN
 
 
 def solve(fg: BoundPICNN, y0, nIter=30, lr=0.01, momentum=0.3, return_device=False):
-    if not isinstance(fg, BoundPICNN):
-        raise TypeError("gd.solve needs a BoundPICNN (PICNN.bind(x)); for arbitrary callables use "
-                        "your framework's own loop")
+    """``fg``: a BoundPICNN or, for the image-completion energy (completion/icnn.back.py:133-147), a
+    BoundConvPICNN."""
+    if not isinstance(fg, (BoundPICNN, BoundConvPICNN)):
+        raise TypeError("gd.solve needs a BoundPICNN (PICNN.bind(x)) or a BoundConvPICNN (ConvPICNN.bind(x)); for "
+                        "arbitrary callables use your framework's own loop")
+    gd_solve = _capi.lib.icnn_conv_gd_solve if isinstance(fg, BoundConvPICNN) else _capi.lib.icnn_gd_solve
     net = fg.net
     dev = net.device
     with torch.cuda.device(dev):
@@ -33,7 +37,7 @@ def solve(fg: BoundPICNN, y0, nIter=30, lr=0.01, momentum=0.3, return_device=Fal
         g = torch.empty_like(y)
         f = torch.empty(fg.B, dtype=torch.float32, device=dev)
         stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _capi.check(_capi.lib.icnn_gd_solve(net._h, C.byref(fg.c_gates), y.data_ptr(), v.data_ptr(),
+        _capi.check(gd_solve(net._h, C.byref(fg.c_gates), y.data_ptr(), v.data_ptr(),
                                             g.data_ptr(), f.data_ptr(), int(nIter), float(lr),
                                             float(momentum), fg.ws.data_ptr(), stream))
         if return_device:

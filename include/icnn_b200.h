@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ICNN_ABI_VERSION 5
+#define ICNN_ABI_VERSION 6
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -267,6 +267,50 @@ int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, const int64_
 size_t icnn_adam_workspace_bytes(int32_t B, int32_t n);
 int icnn_adam_solve(const icnn_picnn_t* h, const icnn_gates* gates, double* act_best, double* f_best,
                     int32_t max_iter, int32_t* iters_out, void* scratch, void* workspace, void* stream);
+
+/* ---- convolutional PICNN (the image-completion energy) ------------------------------------------ */
+/* replaces: the TF graph behind fg() of the completion experiment, Model.f (completion/icnn_ebundle.py:337-452,
+ * = completion/icnn.back.py:276-396) with E_ / dE_dy_ (:118-120).  Images are H x W, y and x are [B, H*W] in
+ * row-major H x W order, feature maps NHWC.  Conv z-layers l = 0..Lc-1 with (C[l], k[l], s[l]) and TensorFlow
+ * 'SAME' padding (H_{l+1} = ceil(H_l / s_l), the odd pad at the end), then dense z-layers of widths fcs[0..Ld-1],
+ * fcs[Ld-1] = 1 (the energy).  Weight layouts are TensorFlow's (host arrays of device pointers):
+ *   Wz[l]   conv l:  [k, k, C_{l-1}, C_l]  ('z{l}_zu_proj/W', >= 0; Wz[0] = NULL)
+ *           dense:   [in, out]             ('z{i}_zu_proj/W', in = flat size of z_{i-1}, NHWC order)
+ *   Wy[l]   [k, k, 1, C_l]  ('z{l}_yu/W'),  Wred[l] [k, k, 1, 1], bred[l] [1]  ('z{l}_y_red/W|b'), l < Lc
+ * The gates are an icnn_gates over Lc + Ld layers (x-path products, computed once per minibatch):
+ *   conv l:   cy[l] [B, H_l, W_l], cz[l] [B, H_l, W_l, C_{l-1}] (cz[0] = NULL), d[l] [B, H_{l+1}, W_{l+1}, C_l]
+ *   dense i:  cy[i] = NULL, cz[i] [B, in_i], d[i] [B, fcs]
+ *   in_scale, in_shift, g_scale must be (1, 0, 1). */
+typedef struct icnn_conv_picnn icnn_conv_picnn_t; /* opaque: packed device copies of the y-path weights */
+typedef struct {
+  int32_t H, W;
+  int32_t Lc;             /* conv z-layers, 1..8                                         */
+  const int32_t* C;       /* host [Lc] output channels                                   */
+  const int32_t* k;       /* host [Lc] kernel sizes                                      */
+  const int32_t* s;       /* host [Lc] strides                                           */
+  int32_t Ld;             /* dense z-layers including the width-1 output, 1..8           */
+  const int32_t* fcs;     /* host [Ld] widths, fcs[Ld-1] = 1                             */
+  const float* const* Wz; /* host [Lc + Ld]                                              */
+  const float* const* Wy; /* host [Lc]                                                   */
+  const float* const* Wred; /* host [Lc]                                                 */
+  const float* const* bred; /* host [Lc]                                                 */
+} icnn_conv_picnn_desc;
+int icnn_conv_picnn_create(const icnn_conv_picnn_desc* desc, icnn_conv_picnn_t** out, void* stream);
+int icnn_conv_picnn_destroy(icnn_conv_picnn_t* h);
+/* bytes of caller-provided device scratch icnn_conv_picnn_fg needs for B rows */
+size_t icnn_conv_picnn_workspace_bytes(const icnn_conv_picnn_t* h, int32_t B);
+/* f and df/dy with the argument list and g-row placement of icnn_picnn_fg (n = H*W). */
+int icnn_conv_picnn_fg(const icnn_conv_picnn_t* h, const icnn_gates* gates, const float* y32, float* f,
+                       float* g, int64_t g_row_stride, const int32_t* perm, const int32_t* count,
+                       int32_t KS, void* workspace, const int32_t* skip_if_zero, void* stream);
+/* replaces: solveBatch (lib/bundle_entropy.py:192-242) as the completion script calls it with this energy
+ * (completion/icnn_ebundle.py:218-226): icnn_bundle_init + nIter x (icnn_conv_picnn_fg, icnn_bundle_step). */
+int icnn_conv_solve_batch_fused(const icnn_conv_picnn_t* h, const icnn_gates* gates, const icnn_bundle_cfg* cfg,
+                                const icnn_bundle_bufs* b, void* workspace, void* stream);
+/* replaces: the unrolled momentum-GD inner loop of completion/icnn.back.py:133-147 on this energy; the
+ * arguments are those of icnn_gd_solve. */
+int icnn_conv_gd_solve(const icnn_conv_picnn_t* h, const icnn_gates* gates, float* y32, float* v, float* g,
+                       float* f_out, int32_t nIter, float lr, float momentum, void* workspace, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------ */
 /* Self test of the wgmma / TMA GEMM the tensor-core K1 path is built from:
