@@ -2,6 +2,7 @@
 // instantiated in bundle_pc_b.cu / bundle_pc_c.cu so that `make -j` compiles them in parallel.
 #include "bundle_pc_kernel.cuh"
 
+#include <cstdio>
 #include <cstdlib>
 
 namespace icnn {
@@ -105,6 +106,14 @@ int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int 
   a.flags = 0;
   if (const char* v = getenv("ICNN_PC_FLAGS")) a.flags = atoi(v);
   if (const char* v = getenv("ICNN_PC_LEGACY")) { if (v[0] == '1') a.flags |= 4; }
+  // L2 prefetch distances of the V3 row sweeps: sweep A one loop trip ahead, sweep B eight rows ahead (chosen per
+  // setting with tools/k2_profile.py at C5 on H100, DESIGN.md §3 "Row passes").  ICNN_PC_PREFETCH="a,b" overrides them
+  // at every launch ("0,0" = off), so settings can be compared in one process.
+  a.pfa = 1; a.pfb = 8;
+  if (const char* v = getenv("ICNN_PC_PREFETCH")) {
+    int pa = 0, pb = 0;
+    if (sscanf(v, "%d,%d", &pa, &pb) == 2 && pa >= 0 && pa <= 8 && pb >= 0 && pb <= 64) { a.pfa = pa; a.pfb = pb; }
+  }
   cudaError_t e;
   const int key = (c.v3 ? 3000 : 0) + (c.gv ? 2000 : 0) + (c.vec ? 0 : 1000) + c.wps * 10 + c.nch;
   switch (key) {

@@ -45,7 +45,13 @@ struct PcArgs {
   int npad;  // doubles reserved per n-vector
   int flags; // exploration knobs (bundle_pc.cu): bit 0 = general k x k stage even for k <= 32, bit 1 = plain stores for xs,
              // bit 2 = sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY)
+  int pfa;   // V3 sweep A: L2 prefetch of the row groups this many loop trips ahead (0 = none)
+  int pfb;   // V3 sweep B: L2 prefetch of the row this many rows ahead (0 = none)
 };
+
+// L2 prefetch of the line holding p (no register is held for it and no result comes back: it only starts the HBM read
+// early).  Used by the row sweeps of the V3 kernel, which are bound by the latency of their row loads.
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 constexpr int PC_NKV = 18;
 constexpr int PC_NKV_V3 = 12;   // V3: tk / ek / rk (append + dependency test, commit) alias dza / dzp / dzq (IPM only)
@@ -202,7 +208,7 @@ __device__ __forceinline__ double dweight(double y) { return fma(-y, y, y); }
 template <int WPS, int NA, int NB, bool TRI, bool PSEUDO, bool VEC, bool GVL, class G>
 __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                               const double* rv, double* Lp, double* qk, double* wk, double* scratch,
-                                              int scap, int a0, int b0) {
+                                              int scap, int a0, int b0, int pfd = 0) {
   constexpr int NT = TRI ? NA * (NA + 1) / 2 : NA * NB;
   constexpr int NL = TRI ? NB : NA + NB;
   double acc[NT][2];
@@ -256,6 +262,16 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
           if (col + 1 < n) v[u][b].y = p[1];
           if (col + 2 < n) v[u][b].z = p[2];
           if (col + 3 < n) v[u][b].w = p[3];
+        }
+      }
+    }
+    if (pfd > 0) {   // the groups of the trip pfd trips ahead: their HBM reads overlap this trip's tensor-core work
+#pragma unroll
+      for (int u = 0; u < NG; ++u) {
+        const int col = (gi + (pfd * NG + u) * WPS) * 16 + 4 * q;
+        if (col < n) {
+#pragma unroll
+          for (int b = 0; b < NL; ++b) if (rok[b]) prefetch_l2(rp[b] + (col - 4 * q));
         }
       }
     }
@@ -368,9 +384,10 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
 
 template <int WPS, int NB, bool VEC, bool GVL, class G>
 __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
-                                                  const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap) {
-  gram_sweep_pc<WPS, 2, NB, false, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4);
-  gram_sweep_pc<WPS, 2, NB, false, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4);
+                                                  const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
+                                                  int pfd) {
+  gram_sweep_pc<WPS, 2, NB, false, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4, pfd);
+  gram_sweep_pc<WPS, 2, NB, false, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4, pfd);
 }
 
 // k + 2 sweep rows in rb = ceil((k + 2) / 8) <= 8 row blocks (k <= 62).  On return warp 0 has stored M0, q, w.
@@ -382,21 +399,21 @@ __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const
 template <int WPS, bool VEC, bool GVL, bool ONE5, class G>
 __device__ __forceinline__ void gram_pass_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                              const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
-                                             bool split5) {
+                                             bool split5, int pfd) {
   const int rb = (k + 2 + 7) >> 3;
-  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
-  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
-  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
+  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   else if (ONE5 && rb == 5 && !split5) {
-    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
+    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   } else {
-    gram_sweep_pc<WPS, 4, 4, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0);
+    gram_sweep_pc<WPS, 4, 4, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
     if (rb > 4) {
       const int r2 = rb - 4;
-      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4); gram_rect_pair_pc<WPS, 1, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap); }
-      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4); gram_rect_pair_pc<WPS, 2, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap); }
-      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4); gram_rect_pair_pc<WPS, 3, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap); }
-      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4); gram_rect_pair_pc<WPS, 4, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap); }
+      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 1, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 2, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 3, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 4, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
     }
   }
 }
@@ -409,7 +426,7 @@ __device__ __forceinline__ int pc_col(int cb, int tid, int c) { return VEC ? cb 
 // UNR: rows per unrolled trip of the row loop = row loads in flight per thread (the pass is bound by them)
 template <int T, int NR, bool VEC, int UNR = 4>
 __device__ __forceinline__ void col_dots_pc(const float* const* rowp, int k, int n, int cb, int tid,
-                                            const double* const (&w)[NR], double (&acc)[NR][4]) {
+                                            const double* const (&w)[NR], double (&acc)[NR][4], int pfr = 0) {
 #pragma unroll
   for (int q = 0; q < NR; ++q)
 #pragma unroll
@@ -420,6 +437,11 @@ __device__ __forceinline__ void col_dots_pc(const float* const* rowp, int k, int
   for (int j = 0; j < k; ++j) {
     const float* p = rowp[j];
     float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (VEC && pfr > 0 && in0) {   // the same columns pfr rows ahead, wrapping into the next chunk after row k - 1
+      const int jp = j + pfr;
+      if (jp < k) prefetch_l2(rowp[jp] + cb + 4 * tid);
+      else if (jp - k < k && cb + 4 * T + 4 * tid < n) prefetch_l2(rowp[jp - k] + cb + 4 * T + 4 * tid);
+    }
     if (VEC) {
       if (in0) { const float4 x = *reinterpret_cast<const float4*>(p + cb + 4 * tid); v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; }
     } else {
@@ -716,7 +738,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     double* zc = PCKV(1 + zsel);
     double* scur = PCKV(3 + zsel);
     // ---- sweep A (warp 0 ends up holding M0, q, w in shared memory)
-    gram_pass_pc<WPS, VEC, GV, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, (A.flags & 4) != 0);
+    gram_pass_pc<WPS, VEC, GV, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, (A.flags & 4) != 0, V3 ? A.pfa : 0);
     // ---- k x k stage
     if (g.warp == 0) {
       const PcKxk io{Lp, invd, zc, scur, wk, hk, qk, dza, dzp, dzq, dsa, sc, isc};
@@ -737,7 +759,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
         const int cb = ch * 4 * T;
         if (cb >= n) break;
         double acc[3][4];
-        col_dots_pc<T, 3, VEC, V3 ? 8 : 4>(rowp, k, n, cb, g.tid, w3, acc);
+        col_dots_pc<T, 3, VEC, V3 ? 8 : 4>(rowp, k, n, cb, g.tid, w3, acc, V3 ? A.pfb : 0);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const int e = pc_col<T, VEC>(cb, g.tid, c);

@@ -26,6 +26,14 @@ BUILDS = {
     "v3off": {"ICNN_PC_V3": "0"},  # 16-warp four-vector kernel, one sample per SM
     "gv8": {"ICNN_PC_GV": "8"},    # n-vectors in global scratch
     "legacy": {"ICNN_PC_LEGACY": "1"},
+    # L2 prefetch distances of the V3 row sweeps, "sweep A trips,sweep B rows" (bundle_pc.cu)
+    "pf0": {"ICNN_PC_PREFETCH": "0,0"},
+    "pfa1": {"ICNN_PC_PREFETCH": "1,0"},
+    "pfa2": {"ICNN_PC_PREFETCH": "2,0"},
+    "pfb8": {"ICNN_PC_PREFETCH": "0,8"},
+    "pfb16": {"ICNN_PC_PREFETCH": "0,16"},
+    "pfa1b8": {"ICNN_PC_PREFETCH": "1,8"},
+    "pfa2b16": {"ICNN_PC_PREFETCH": "2,16"},
 }
 KNOBS = sorted({k for e in BUILDS.values() for k in e})
 PASSES_OUTSIDE = int(os.environ.get("K2_PASSES_OUTSIDE", "5"))
