@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 NSTAT = 8
 
 # status / enum mirrors of include/icnn_b200.h
@@ -63,7 +63,7 @@ class BundleBufs(C.Structure):
                 ("gram", C.c_void_p), ("perm", C.c_void_p), ("count", C.c_void_p),
                 ("status", C.c_void_p), ("finished", C.c_void_p), ("nIters", C.c_void_p),
                 ("nactive", C.c_void_p), ("newton_its", C.c_void_p), ("ksum", C.c_void_p),
-                ("f64", C.c_void_p), ("iter_stats", C.c_void_p), ("vec_ws", C.c_void_p)]
+                ("f64", C.c_void_p), ("iter_stats", C.c_void_p)]
 
 
 class BundleCfg(C.Structure):

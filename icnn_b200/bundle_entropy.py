@@ -95,17 +95,12 @@ class BundleState:
         # optional: float64 f of a float64 callback fg; per-iteration statistics (include/icnn_b200.h)
         self.f64 = e(B, dtype=f64) if keep_f64 else None
         self.iter_stats = torch.zeros(nIter, _capi.NSTAT, dtype=torch.float64, device=device) if stats else None
-        # scratch for the measured-and-rejected variant of the predictor-corrector kernel that keeps the per-sample
-        # n-vectors in L2 instead of shared memory (include/icnn_b200.h: vec_ws): only
-        # allocated when the exploration knob ICNN_PC_GV is set
-        import os
-        self.vec_ws = e(B, 4, (n + 15) & ~15, dtype=f64) if os.environ.get("ICNN_PC_GV") else None
         p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         self.c = _capi.BundleBufs(self.B, self.n, self.KS, p(self.y), p(self.y32), p(self.f), p(self.G),
                                   p(self.ys), p(self.h), p(self.lam), p(self.rsum), p(self.gram),
                                   p(self.perm), p(self.count), p(self.status), p(self.finished),
                                   p(self.nIters), p(self.nactive), p(self.newton_its), p(self.ksum),
-                                  p(self.f64), p(self.iter_stats), p(self.vec_ws))
+                                  p(self.f64), p(self.iter_stats))
         self._host = None
         self._pin_y = None
         self._graphs = {}   # captured device loops (solveBatch(graph=True)), keyed on everything the capture bakes in

@@ -1,8 +1,5 @@
-// K2 predictor-corrector path: instantiations for 4 and 8 warps per sample (see bundle_pc.cu).
+// K2 predictor-corrector path: instantiation for 8 warps per sample (see bundle_pc.cu).
 #include "bundle_pc_kernel.cuh"
 namespace icnn {
-cudaError_t launch_pc_4_1(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<4, 1, true>(a, c, B, st); }
-cudaError_t launch_pc_4_2(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<4, 2, true>(a, c, B, st); }
-cudaError_t launch_pc_8_1(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<8, 1, true>(a, c, B, st); }
-cudaError_t launch_pc_8_2(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<8, 2, true>(a, c, B, st); }
+cudaError_t launch_pc_8x2(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<8, 2, true>(a, c, B, st); }
 }  // namespace icnn

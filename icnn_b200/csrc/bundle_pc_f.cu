@@ -1,7 +1,6 @@
-// K2 predictor-corrector path: three-n-vector instantiations (V3, see bundle_pc_kernel.cuh): two 8-warp samples
-// per SM at n_y = 4096 (C5), three 4-warp samples at n_y = 2048.
+// K2 predictor-corrector path: the three-n-vector instantiation (V3, see bundle_pc_kernel.cuh): two 8-warp samples
+// per SM at n_y = 4096 (C5).
 #include "bundle_pc_kernel.cuh"
 namespace icnn {
-cudaError_t launch_pc_308_4(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<8, 4, true, false, true>(a, c, B, st); }
-cudaError_t launch_pc_304_4(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<4, 4, true, false, true>(a, c, B, st); }
+cudaError_t launch_pc_v3_8x4(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) { return launch_pc<8, 4, true, true>(a, c, B, st); }
 }  // namespace icnn

@@ -43,10 +43,9 @@ struct PcArgs {
   icnn_bundle_cfg c;
   int t;
   int npad;  // doubles reserved per n-vector
-  int flags; // exploration knobs (bundle_pc.cu): bit 0 = general k x k stage even for k <= 32, bit 1 = plain stores for xs,
-             // bit 2 = sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY)
   int pfa;   // V3 sweep A: L2 prefetch of the row groups this many loop trips ahead (0 = none)
   int pfb;   // V3 sweep B: L2 prefetch of the row this many rows ahead (0 = none)
+  bool split5;  // sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY=1, see gram_pass_pc)
 };
 
 // L2 prefetch of the line holding p (no register is held for it and no result comes back: it only starts the HBM read
@@ -56,8 +55,8 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 constexpr int PC_NKV = 18;
 constexpr int PC_NKV_V3 = 12;   // V3: tk / ek / rk (append + dependency test, commit) alias dza / dzp / dzq (IPM only)
 
-__host__ __device__ inline size_t pc_group_doubles(int npad, int KS, int wps, bool gv = false, bool v3 = false) {
-  size_t d = (gv ? (size_t)0 : (size_t)(v3 ? 3 : 4) * npad) + (size_t)KS * (KS + 1) / 2 +
+__host__ __device__ inline size_t pc_group_doubles(int npad, int KS, int wps, bool v3) {
+  size_t d = (size_t)(v3 ? 3 : 4) * npad + (size_t)KS * (KS + 1) / 2 +
              (size_t)(v3 ? PC_NKV_V3 : PC_NKV) * KS + KS /* row pointers */ +
              8 * wps /* two reduction buffers */ + 16 /* scalars */ + 4 /* 8 ints */;
   return (d + 1) & ~(size_t)1;
@@ -205,7 +204,7 @@ __device__ __forceinline__ double dweight(double y) { return fma(-y, y, y); }
 // values, so only the loads of G are predicated.  The warp partials are summed by a fixed tree through a
 // scratch n-vector (deterministic), and warp 0 stores the result (packed matrix / q / w).
 // VEC: rows are 16-byte aligned (n % 4 == 0) -> one 128-bit load per row block.
-template <int WPS, int NA, int NB, bool TRI, bool PSEUDO, bool VEC, bool GVL, class G>
+template <int WPS, int NA, int NB, bool TRI, bool PSEUDO, bool VEC, class G>
 __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                               const double* rv, double* Lp, double* qk, double* wk, double* scratch,
                                               int scap, int a0, int b0, int pfd = 0) {
@@ -235,22 +234,12 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
 #pragma unroll 1
   for (int gi = g.warp; gi < ngrp; gi += NG * WPS) {
     float4 v[NG][NL];
-    double2 yl[GVL ? NG : 1][2], rl[GVL ? NG : 1][2];   // GVL: y / ry come from L2 as well -> issued with the row loads
 #pragma unroll
     for (int u = 0; u < NG; ++u) {
       const int gu = gi + u * WPS;
       const int off = gu * 16;
       const int col = off + 4 * q;
       const bool gv = (u == 0) || gu < ngrp;
-      if (GVL) {
-        const int og = gv ? off : 0;
-        yl[GVL ? u : 0][0] = *reinterpret_cast<const double2*>(yq + og);
-        yl[GVL ? u : 0][1] = *reinterpret_cast<const double2*>(yq + og + 2);
-        if (PSEUDO && ps && r == 0) {
-          rl[GVL ? u : 0][0] = *reinterpret_cast<const double2*>(rq + og);
-          rl[GVL ? u : 0][1] = *reinterpret_cast<const double2*>(rq + og + 2);
-        }
-      }
 #pragma unroll
       for (int b = 0; b < NL; ++b) {
         v[u][b] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -280,14 +269,14 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
       const int gu = gi + u * WPS;
       if (u > 0 && gu >= ngrp) break;
       const int off = gu * 16;
-      const double2 ya = GVL ? yl[GVL ? u : 0][0] : *reinterpret_cast<const double2*>(yq + off);
-      const double2 yb = GVL ? yl[GVL ? u : 0][1] : *reinterpret_cast<const double2*>(yq + off + 2);
+      const double2 ya = *reinterpret_cast<const double2*>(yq + off);
+      const double2 yb = *reinterpret_cast<const double2*>(yq + off + 2);
       double dd[4] = {dweight(ya.x), dweight(ya.y), dweight(yb.x), dweight(yb.y)};
       double pa[4] = {0.0, 0.0, 0.0, 0.0};
       if (PSEUDO && ps) {
         if (r == 0) {
-          const double2 ra = GVL ? rl[GVL ? u : 0][0] : *reinterpret_cast<const double2*>(rq + off);
-          const double2 rb = GVL ? rl[GVL ? u : 0][1] : *reinterpret_cast<const double2*>(rq + off + 2);
+          const double2 ra = *reinterpret_cast<const double2*>(rq + off);
+          const double2 rb = *reinterpret_cast<const double2*>(rq + off + 2);
           pa[0] = dd[0] * ra.x; pa[1] = dd[1] * ra.y; pa[2] = dd[2] * rb.x; pa[3] = dd[3] * rb.y;
         } else {
           pa[0] = ya.x; pa[1] = ya.y; pa[2] = yb.x; pa[3] = yb.y;
@@ -382,12 +371,12 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
   }
 }
 
-template <int WPS, int NB, bool VEC, bool GVL, class G>
+template <int WPS, int NB, bool VEC, class G>
 __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                                   const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
                                                   int pfd) {
-  gram_sweep_pc<WPS, 2, NB, false, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4, pfd);
-  gram_sweep_pc<WPS, 2, NB, false, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4, pfd);
+  gram_sweep_pc<WPS, 2, NB, false, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4, pfd);
+  gram_sweep_pc<WPS, 2, NB, false, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4, pfd);
 }
 
 // k + 2 sweep rows in rb = ceil((k + 2) / 8) <= 8 row blocks (k <= 62).  On return warp 0 has stored M0, q, w.
@@ -396,24 +385,24 @@ __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const
 // accumulators in one sweep would spill).  ONE5 (V3 build only: the other builds have no register room for 15 tiles)
 // enables the one-sweep rb = 5, which at C5 carries the last outer iterations (k = 31..38); split5 sends rb = 5 through
 // the composition anyway (11 block loads instead of 5; ICNN_PC_LEGACY=1, the form the one sweep is tested against).
-template <int WPS, bool VEC, bool GVL, bool ONE5, class G>
+template <int WPS, bool VEC, bool ONE5, class G>
 __device__ __forceinline__ void gram_pass_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                              const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
                                              bool split5, int pfd) {
   const int rb = (k + 2 + 7) >> 3;
-  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
-  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
-  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   else if (ONE5 && rb == 5 && !split5) {
-    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   } else {
-    gram_sweep_pc<WPS, 4, 4, true, true, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+    gram_sweep_pc<WPS, 4, 4, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
     if (rb > 4) {
       const int r2 = rb - 4;
-      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 1, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 2, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 3, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 4, VEC, GVL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 1, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 2, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 3, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 4, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
     }
   }
 }
@@ -521,12 +510,8 @@ __device__ __forceinline__ void pc_kxk_stage(const PcKxk& io, int k, int lane, d
 // One CTA of WPS warps per sample (the block scheduler balances the SMs at sample granularity: with several
 // samples per CTA the last, partly filled wave costs a whole extra round);  NCH = chunks of 4 T columns per
 // thread (n <= 4 T NCH);  R80: 80-register build (768 threads / SM) instead of 128 registers (512 / SM).
-// GV: the four n-vectors of a sample live in the caller's scratch (icnn_bundle_bufs::vec_ws, L2-resident) instead of
-// shared memory: shared memory per sample drops to the k x k part, so the samples in flight per SM are bounded by
-// registers / threads only and the one-warp k x k stage of one sample overlaps the sweeps of the others.
-template <int WPS, int NCH, bool R80, bool VEC, bool GV = false, bool V3 = false>
+template <int WPS, int NCH, bool R80, bool VEC, bool V3>
 __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WPS) bundle_pc_kernel(PcArgs A) {
-  static_assert(!(GV && V3), "V3 is a shared-memory layout");
   const icnn_bundle_bufs& b = A.b;
   const icnn_bundle_cfg& cf = A.c;
   if (b.nactive[A.t] == 0) return;
@@ -534,7 +519,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   constexpr int GPB = 1;
   constexpr int T = WPS * 32;
   static_assert(NCH == 1 || NCH == 2 || NCH == 4, "NCH");
-  Grp<WPS, 1> g;
+  Grp<WPS> g;
   g.tid = threadIdx.x % T;
   g.lane = threadIdx.x & 31;
   g.warp = g.tid >> 5;
@@ -544,12 +529,12 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   if (b.finished[u]) return;
 
   const int n = b.n, KS = b.KS, npad = A.npad;
-  double* base = smem_d + (size_t)g.gid * pc_group_doubles(npad, KS, WPS, GV, V3);
-  double* yv = GV ? b.vec_ws + (size_t)u * 4 * npad : base;
+  double* base = smem_d + (size_t)g.gid * pc_group_doubles(npad, KS, WPS, V3);
+  double* yv = base;
   double* uv = V3 ? nullptr : yv + npad;   // V3: u is not stored (recovered as ry - logit(y) in the update)
   double* rv = V3 ? yv + npad : uv + npad;   // ry, then du (V3: ry only)
   double* xv = rv + npad;   // v1 + v3, then dy (V3: then du) ; scratch of the dependency test and of the sweep-A tree sum
-  double* Lp = GV ? base : xv + npad;   // packed lower k x k
+  double* Lp = xv + npad;   // packed lower k x k
   double* kv = Lp + (size_t)KS * (KS + 1) / 2;
 #define PCKV(i) (kv + (i) * KS)
   double* hk = PCKV(0);
@@ -601,7 +586,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       hs = fma(ge, ye, hs);
       rs += ge;
       if (!isfinite(ge)) bad = 1.0;
-      if (ysrow) { if (A.flags & 2) ysrow[e] = ye; else __stcs(ysrow + e, ye); }   // write-only during the solve: streaming store
+      if (ysrow) __stcs(ysrow + e, ye);   // write-only during the solve: streaming store
       if (b.iter_stats) ent += neg_entropy(ye);
     }
     if (b.iter_stats) ent = g.sum(ent);
@@ -738,11 +723,11 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     double* zc = PCKV(1 + zsel);
     double* scur = PCKV(3 + zsel);
     // ---- sweep A (warp 0 ends up holding M0, q, w in shared memory)
-    gram_pass_pc<WPS, VEC, GV, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, (A.flags & 4) != 0, V3 ? A.pfa : 0);
+    gram_pass_pc<WPS, VEC, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, A.split5, V3 ? A.pfa : 0);
     // ---- k x k stage
     if (g.warp == 0) {
       const PcKxk io{Lp, invd, zc, scur, wk, hk, qk, dza, dzp, dzq, dsa, sc, isc};
-      if (k <= 32 && !(A.flags & 1)) pc_kxk_stage<true>(io, k, g.lane, pr);
+      if (k <= 32) pc_kxk_stage<true>(io, k, g.lane, pr);
       else pc_kxk_stage<false>(io, k, g.lane, pr);
     }
     g.sync();
@@ -910,14 +895,14 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
 #undef PCKV
 }
 
-struct PcConfig { int wps, nch, npad, minb; bool vec, gv, v3; size_t smem; };
+struct PcConfig { int wps, nch, npad, minb; bool vec, v3; size_t smem; };
 
-template <int WPS, int NCH, bool VEC, bool GV = false, bool V3 = false>
+template <int WPS, int NCH, bool VEC, bool V3 = false>
 static cudaError_t launch_pc(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) {
   void (*kern)(PcArgs);
-  if constexpr (V3) kern = bundle_pc_kernel<WPS, NCH, false, VEC, false, true>;   // 128-register build, two CTAs per SM
-  else if constexpr (WPS == 16) kern = bundle_pc_kernel<16, NCH, false, VEC, GV>;
-  else kern = (c.minb >= 3) ? bundle_pc_kernel<WPS, NCH, true, VEC, GV> : bundle_pc_kernel<WPS, NCH, false, VEC, GV>;
+  // V3: 128-register build, two CTAs per SM; 1 and 16 warps per sample: the 128-register build only (pc_fits)
+  if constexpr (V3 || WPS == 16 || WPS == 1) kern = bundle_pc_kernel<WPS, NCH, false, VEC, V3>;
+  else kern = (c.minb >= 3) ? bundle_pc_kernel<WPS, NCH, true, VEC, false> : bundle_pc_kernel<WPS, NCH, false, VEC, false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem);
   if (e != cudaSuccess) return e;
   if constexpr (V3) {   // the whole point is two 113 KB samples per SM: ask for the largest shared-memory carve-out

@@ -26,7 +26,8 @@
 extern "C" {
 #endif
 
-#define ICNN_ABI_VERSION 6
+/* 7: icnn_bundle_bufs ends at iter_stats (the vec_ws scratch pointer of version 6 is gone; 19 pointers) */
+#define ICNN_ABI_VERSION 7
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -109,9 +110,6 @@ typedef struct {
                         [5] samples stopped in this iteration (rank / convergence / non-finite)
                         [6] sum of f(y_t) - H(y_t) over the samples entering the iteration (0 log 0 = 0)
                         [7] reserved                                                                  */
-  double* vec_ws;    /* optional (may be NULL): device scratch of B * 4 * ((n + 15) & ~15) doubles.  When set, the
-                        predictor-corrector kernel may keep a sample's four n-vectors (y, u, ry, dy) there (L2-resident)
-                        instead of in shared memory, which multiplies the samples in flight per SM (DESIGN.md K2)    */
 } icnn_bundle_bufs;
 #define ICNN_NSTAT 8
 

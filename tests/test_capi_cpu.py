@@ -25,7 +25,7 @@ def test_library_exports_every_header_symbol():
 def test_struct_layouts_match_header_sizes():
     from icnn_b200 import _capi
     # 3 int32 (+pad) + 17 pointers ; cfg: 4 int32 + 2 double + 2 int32
-    assert C.sizeof(_capi.BundleBufs) == 16 + 20 * 8   # 3 int32 (+pad) + 20 pointers (ABI v2: + f64, iter_stats, vec_ws)
+    assert C.sizeof(_capi.BundleBufs) == 16 + 19 * 8   # 3 int32 (+pad) + 19 pointers (ABI v7: ends at f64, iter_stats)
     assert C.sizeof(_capi.BundleCfg) == 16 + 16 + 8
     assert C.sizeof(_capi.Gates) == 8 + 3 * 8 + 12 + 4
     assert C.sizeof(_capi.PicnnDesc) == 8 + 8 + 8 + 8 + 8

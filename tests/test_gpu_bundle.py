@@ -65,10 +65,27 @@ def lens(rows):
 K2_CASES = [("C1", 64, 5), ("C1", 13, 20), ("C3", 24, 10), ("T", 12, 10), ("C5", 3, 6)]
 
 
-@pytest.mark.parametrize("name,B,nIter", K2_CASES)
+def _shape(n, hidden, seed):
+    """A small-network workload at n_y = n: what K2 launches depends on (n_y, nIter) only."""
+    return dict(synth.CONFIGS["C3"], m=64, n=n, hidden=hidden, seed=seed)
+
+
+# The builds of the two-sweep PC kernel that no named workload reaches.  With the cases above (C3: one warp, two column
+# chunks, scalar row loads; C5: three-vector build) and the C2 golden cases (8 warps) every build bundle_pc.cu selects
+# is compared with the oracle.
+K2_PC_SHAPES = [
+    pytest.param(_shape(100, [96, 64], 11), 24, 10, id="n100-1warp-1chunk"),
+    pytest.param(_shape(90, [96, 64], 11), 24, 10, id="n90-1warp-1chunk-scalar"),
+    pytest.param(_shape(200, [96, 64], 11), 24, 10, id="n200-1warp-2chunks"),
+    # 57 slots at n_y = 4096: two three-vector samples no longer fit an SM -> four-vector build, 16 warps, 2 chunks
+    pytest.param(_shape(4096, [96, 64], 11), 24, 56, id="n4096-57slots-16warps-2chunks"),
+    pytest.param(_shape(5000, [256, 128], 12), 24, 10, id="n5000-16warps-4chunks"),
+]
+
+
+@pytest.mark.parametrize("name,B,nIter", K2_CASES + K2_PC_SHAPES)
 def test_k2_pc_matches_oracle(name, B, nIter):
     from icnn_b200 import bundle_entropy as be
-    cfg = synth.CONFIGS[name]
     p, x, y0 = synth.make_inputs(name, B=B)
     fg = r32(picnn_np.make_fg(p, x))
     o = bundle_np.solve_batch(fg, y0.copy(), nIter=nIter, variant="lib", solver="pc")
@@ -479,7 +496,6 @@ def test_resident_cluster_variant_matches_streaming(name, B, nIter, env, monkeyp
 @pytest.mark.parametrize("name,B,nIter,env_ref,env_alt", [
     ("C5", 3, 12, {"ICNN_PC_V3": "0"}, {}),                  # n_y = 4096: three-vector build is the default
     ("C5", 3, 45, {"ICNN_PC_V3": "0"}, {}),                  # deep horizon: k up to ~35 rows, every row-block shape of sweep A
-    ("C2", 5, 14, {}, {"ICNN_PC_V3": "1"}),                  # n_y = 2048: forced three-vector build vs the five-sweep default
 ])
 def test_three_vector_pc_kernel_matches_four_vector(name, B, nIter, env_ref, env_alt, monkeypatch):
     """The V3 build of the predictor-corrector kernel (y, ry, du in shared memory; u = ry - logit(y) and dy recomputed

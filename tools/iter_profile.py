@@ -38,7 +38,7 @@ for rep in range(2):
             cnt = st.count.cpu().numpy(); fin = st.finished.cpu().numpy(); ni = int(st.newton_its.cpu().numpy().sum())
             stats.append((cnt.mean(), cnt.max(), int((fin == 0).sum()), ni - (stats[-1][4] if stats else 0), ni))
     torch.cuda.synchronize()
-print("%s B=%d n=%d nIter=%d solver=%s WPS=%s MINB=%s" % (name, B, n, nIter, solver, os.environ.get("ICNN_K2_WPS", "auto"), os.environ.get("ICNN_K2_MINB", "3")))
+print("%s B=%d n=%d nIter=%d solver=%s WPS=%s" % (name, B, n, nIter, solver, os.environ.get("ICNN_K2_WPS", "auto")))
 k1 = [a.elapsed_time(b) for a, b, _ in evs]; k2 = [b.elapsed_time(c) for _, b, c in evs]
 for t in range(nIter):
     if t < 6 or t % 5 == 4 or t == nIter - 1:

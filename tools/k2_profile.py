@@ -1,7 +1,7 @@
 """K2 alone at a workload (default C5), per outer iteration t, for several builds of the bundle step (exploration
 tool, not part of bench.py).
 
-    python tools/k2_profile.py [--workload C5] [--reps 2] [--builds v3,v3off,gv8] [--json OUT]
+    python tools/k2_profile.py [--workload C5] [--reps 2] [--builds v3,v3off] [--json OUT]
 
 The bundle loop is driven through the per-iteration entries (icnn_bundle_init, icnn_picnn_fg, icnn_bundle_step) as in
 bench.py's instrumented pass, and only the K2 launch of each t is timed (CUDA events).  The build is picked by the
@@ -24,7 +24,6 @@ import torch  # noqa: E402
 BUILDS = {
     "v3": {},                      # the default at 2048 < n_y <= 4096
     "v3off": {"ICNN_PC_V3": "0"},  # 16-warp four-vector kernel, one sample per SM
-    "gv8": {"ICNN_PC_GV": "8"},    # n-vectors in global scratch
     "legacy": {"ICNN_PC_LEGACY": "1"},
     # L2 prefetch distances of the V3 row sweeps, "sweep A trips,sweep B rows" (bundle_pc.cu)
     "pf0": {"ICNN_PC_PREFETCH": "0,0"},
@@ -43,7 +42,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="C5")
     ap.add_argument("--reps", type=int, default=2)
-    ap.add_argument("--builds", default="v3,v3off,gv8")
+    ap.add_argument("--builds", default="v3,v3off")
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     import icnn_b200
@@ -60,10 +59,7 @@ def main():
     ccfg = bundle_entropy._make_cfg(cfg["variant"], "pc", nIter, None, None, 0, n, KS)
     for k in KNOBS:
         os.environ.pop(k, None)
-    if "gv8" in builds:
-        os.environ["ICNN_PC_GV"] = "8"   # BundleState allocates the global n-vector scratch only when this is set
     st = bundle_entropy.BundleState(B, n, KS, dev, keep_xs=True, nIter=nIter, stats=True)
-    os.environ.pop("ICNN_PC_GV", None)
     stats_ptr = st.c.iter_stats
     y0d = torch.from_numpy(y0).to(dev)
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)

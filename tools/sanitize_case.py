@@ -1,7 +1,7 @@
 """Small end-to-end cases for compute-sanitizer (memcheck / racecheck / synccheck):
     compute-sanitizer --tool racecheck python tools/sanitize_case.py
-Covers K1 FFMA + cluster split-K, K1 wgmma path, K2 group kernel (WPS 1/2/8, PC + dual + RL Newton),
-K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the wgmma path (pitch-padded
+Covers K1 FFMA + cluster split-K, K1 wgmma path, K2 five-sweep group kernel (1 / 2 / 8 warps per sample, PC + dual +
+RL Newton), every build of the K2 two-sweep PC kernel the dispatch selects, K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the wgmma path (pitch-padded
 operands), GD training backward (FFMA and wgmma GDB instantiation, split-K weight-gradient GEMM)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -48,16 +48,21 @@ if "gdgrad" in which:
         yN, gr = icnn_b200.gd_grad.gd_grad(icnn_b200.PICNN.from_params(p).bind(x), np.full((B, dims[1]), 0.5), tY,
                                            nIter=3, lr=0.02, momentum=0.5, x=x)
         print("gdgrad ok", dims, B, float(np.abs(gr["Wy"][0]).max()), flush=True)
-if "pc" in which:     # round 2: the two-sweep PC kernel in every group size, both alignments, the > 4 row-block sweeps, and
-    # the chunked-accumulation wgmma GEMM (T, 64 rows above)
-    run("C3", 5, 5)                                     # 1 warp / sample, n_y % 4 != 0 (scalar row loads)
-    for w in ("1", "2", "4", "8"):
-        os.environ["ICNN_PC_WPS"] = w
-        run("T", 3, 4)                                  # n_y = 512 on 1 / 2 / 4 / 8 warps per sample
-    os.environ["ICNN_PC_WPS"] = "2"
-    run("T", 2, 36)                                     # k + 2 > 32 sweep rows: second triangle + rectangle sweeps
-    os.environ.pop("ICNN_PC_WPS")
-    run("C5", 2, 6)                                     # 16 warps / sample (n_y = 4096)
+if "pc" in which:     # the two-sweep PC kernel in every build bundle_pc.cu selects, both alignments, the > 4 row-block sweeps
+    def pc_shape(n, B, nIter):
+        p = workloads.synth_params(5, 16, n, [32, 32])
+        x = np.random.RandomState(3).randn(B, 16)
+        out = be.solveBatch(icnn_b200.PICNN.from_params(p).bind(x), np.full((B, n), 0.5), nIter=nIter)
+        print("pc n_y", n, B, nIter, "ok, y range", float(out[0].min()), float(out[0].max()), flush=True)
+    pc_shape(100, 5, 5)                                 # 1 warp / sample, 1 chunk
+    pc_shape(90, 5, 5)                                  # the same with n_y % 4 != 0 (scalar row loads)
+    pc_shape(200, 5, 5)                                 # 1 warp / sample, 2 chunks
+    run("C3", 5, 5)                                     # the same with n_y % 4 != 0
+    run("C3", 2, 36)                                    # k + 2 > 32 sweep rows: second triangle + rectangle sweeps
+    run("C2", 2, 4)                                     # 8 warps / sample (n_y = 2048)
+    run("C5", 2, 6)                                     # three-vector build, 8 warps / sample (n_y = 4096)
+    run("C5", 2, 56)                                    # 16 warps / sample, 2 chunks: KS too large for two samples per SM
+    pc_shape(5000, 2, 4)                                # 16 warps / sample, 4 chunks
     _, _, o = run("C3", 4, 4, stats=True)
     print("stats", o[-1].stats()["entering"], flush=True)
 print("done")
