@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
 ABI_VERSION = 7
 NSTAT = 8
+K2_PLAN_LEN = 8     # ICNN_K2_PLAN_LEN: int32 fields of an icnn_k2_plan / icnn_k2_last_launch record
 
 # status / enum mirrors of include/icnn_b200.h
 ST_RUNNING, ST_RANK_STOP, ST_SOLVE_FAIL, ST_NONFINITE, ST_CONVERGED = 0, 2, 3, 4, 5
@@ -31,7 +32,7 @@ SYMBOLS = [
     "icnn_adam_workspace_bytes", "icnn_adam_solve",
     "icnn_gd_backward_workspace_bytes", "icnn_gd_backward", "icnn_fp64_mma_probe",
     "icnn_loop_graph_create", "icnn_loop_graph_launch", "icnn_loop_graph_nodes", "icnn_loop_graph_destroy",
-    "icnn_tc_set_tuning", "icnn_tc_last_launch",
+    "icnn_tc_set_tuning", "icnn_tc_last_launch", "icnn_k2_plan", "icnn_k2_last_launch",
     "icnn_train_grad_workspace_bytes", "icnn_train_grad",
     "icnn_conv_picnn_create", "icnn_conv_picnn_destroy", "icnn_conv_picnn_workspace_bytes", "icnn_conv_picnn_fg",
     "icnn_conv_solve_batch_fused", "icnn_conv_gd_solve",
@@ -112,6 +113,8 @@ def _load():
                                           C.c_void_p, C.c_void_p]
     lib.icnn_tc_set_tuning.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.icnn_tc_last_launch.argtypes = [C.POINTER(C.c_int32)]
+    lib.icnn_k2_plan.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
+    lib.icnn_k2_last_launch.argtypes = [C.POINTER(C.c_int32)]
     lib.icnn_picnn_set_xpath.argtypes = [C.c_void_p, C.c_int32] + [_fpp] * 8 + [C.c_void_p]
     lib.icnn_picnn_gates_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
     lib.icnn_picnn_gates_workspace_bytes.restype = C.c_size_t

@@ -151,10 +151,15 @@ int argmin_grad_launch(const icnn_bundle_bufs* b, int loss, const double* trueY,
   a.npad = (b->n + 3) & ~3;
   a.ld = (b->KS + 1) | 1;
   const int n = b->n;
-  const int wps = n <= 128 ? 1 : (n <= 512 ? 2 : (n <= 1024 ? 4 : 8));
+  int wps = n <= 128 ? 1 : (n <= 512 ? 2 : (n <= 1024 ? 4 : 8));
   const int KA = b->KS + 1;
-  const size_t per = (((size_t)3 * a.npad + (size_t)2 * KA * a.ld + 4 * KA + 4 * wps + 8 + 1) & ~(size_t)1);
-  const size_t smem = sizeof(double) * per * (8 / wps);
+  auto smem_of = [&](int w) {
+    return sizeof(double) * ((((size_t)3 * a.npad + (size_t)2 * KA * a.ld + 4 * KA + 4 * w + 8 + 1) & ~(size_t)1)) * (8 / w);
+  };
+  // 8 / wps samples share a CTA: when their k x k systems do not fit side by side (large KS at small n_y), the
+  // sample gets more warps and the CTA fewer samples
+  while (wps < 8 && smem_of(wps) > 227 * 1024) wps *= 2;
+  const size_t smem = smem_of(wps);
   if (smem > 227 * 1024) { set_error("argmin_grad: shared memory %zu B exceeds 227 KB", smem); return ICNN_E_UNSUPPORTED; }
   void (*kern)(GradArgs) = wps == 1 ? argmin_grad_kernel<1> : wps == 2 ? argmin_grad_kernel<2> : wps == 4 ? argmin_grad_kernel<4> : argmin_grad_kernel<8>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -39,14 +39,14 @@ static PcTestEnv pc_test_env() {
 }
 
 // The thread that owns a column in sweep B keeps v2 in registers, so n <= 128 * WPS * NCH.
-static bool pc_fits(const icnn_bundle_bufs* b, int wps, int nch, bool v3, PcConfig* out) {
-  if (b->n > 128 * wps * nch) return false;
+static bool pc_fits(int n, int KS, int wps, int nch, bool v3, PcConfig* out) {
+  if (n > 128 * wps * nch) return false;
   PcConfig c;
   c.wps = wps; c.nch = nch; c.v3 = v3;
-  c.npad = (b->n + 15) & ~15;   // the tensor-core sweep reads whole 16-column groups of the n-vectors
-  c.vec = (b->n & 3) == 0;
+  c.npad = (n + 15) & ~15;   // the tensor-core sweep reads whole 16-column groups of the n-vectors
+  c.vec = (n & 3) == 0;
   if (!c.vec && wps > 1) return false;
-  c.smem = sizeof(double) * pc_group_doubles(c.npad, b->KS, wps, v3);
+  c.smem = sizeof(double) * pc_group_doubles(c.npad, KS, wps, v3);
   if (c.smem > 227 * 1024) return false;
   if (v3) {   // only worth it when at least two samples fit an SM (228 KB, 1 KB reserved per CTA)
     if (!c.vec || 2 * (c.smem + 1024) > 228 * 1024) return false;
@@ -67,23 +67,22 @@ static bool pc_fits(const icnn_bundle_bufs* b, int wps, int nch, bool v3, PcConf
 //   1024 < n_y <= 2048   8 warps, 2 chunks   (n_y % 4 == 0, else five-sweep)
 //   2048 < n_y <= 4096   V3: 8 warps, 4 chunks when two samples fit an SM, else 16 warps, 2 chunks
 //   4096 < n_y           16 warps, 4 chunks
-// false: the shape takes the five-sweep kernel (also whenever shared memory does not fit).
-static bool pick_pc(const icnn_bundle_bufs* b, bool allow_v3, PcConfig* out) {
-  const int n = b->n;
-  if (b->KS > 62) return false;   // k + 2 sweep rows in <= 8 row blocks
-  if (n <= 128) return pc_fits(b, 1, 1, false, out);
-  if (n <= 256) return pc_fits(b, 1, 2, false, out);
+// false: the shape takes the five-sweep kernel (also whenever shared memory does not fit).  Part of k2_plan
+// (bundle_step.cu), which reads ICNN_K2_PC first.
+bool pick_pc(int n, int KS, PcConfig* out) {
+  const bool allow_v3 = pc_test_env().v3;
+  if (KS > 62) return false;   // k + 2 sweep rows in <= 8 row blocks
+  if (n <= 128) return pc_fits(n, KS, 1, 1, false, out);
+  if (n <= 256) return pc_fits(n, KS, 1, 2, false, out);
   if (n <= 1024) return false;
-  if (n <= 2048) return pc_fits(b, 8, 2, false, out);
-  if (n <= 4096) return (allow_v3 && pc_fits(b, 8, 4, true, out)) || pc_fits(b, 16, 2, false, out);
-  return pc_fits(b, 16, 4, false, out);
+  if (n <= 2048) return pc_fits(n, KS, 8, 2, false, out);
+  if (n <= 4096) return (allow_v3 && pc_fits(n, KS, 8, 4, true, out)) || pc_fits(n, KS, 16, 2, false, out);
+  return pc_fits(n, KS, 16, 4, false, out);
 }
 
-// returns ICNN_E_UNSUPPORTED when the shape has to take the five-sweep kernel of bundle_step_kernel.cuh
-int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int t, cudaStream_t st) {
+// enqueues the two-sweep build c (from pick_pc)
+int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int t, const PcConfig& c, cudaStream_t st) {
   const PcTestEnv env = pc_test_env();
-  PcConfig c;
-  if (!pick_pc(b, env.v3, &c)) return ICNN_E_UNSUPPORTED;
   PcArgs a;
   a.b = *b; a.c = *cfg; a.t = t; a.npad = c.npad;
   a.split5 = env.split5; a.pfa = env.pfa; a.pfb = env.pfb;

@@ -895,14 +895,13 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
 #undef PCKV
 }
 
-struct PcConfig { int wps, nch, npad, minb; bool vec, v3; size_t smem; };
-
+// (PcConfig, pc_r80: k2_dispatch.cuh)
 template <int WPS, int NCH, bool VEC, bool V3 = false>
 static cudaError_t launch_pc(const PcArgs& a, const PcConfig& c, int B, cudaStream_t st) {
   void (*kern)(PcArgs);
   // V3: 128-register build, two CTAs per SM; 1 and 16 warps per sample: the 128-register build only (pc_fits)
   if constexpr (V3 || WPS == 16 || WPS == 1) kern = bundle_pc_kernel<WPS, NCH, false, VEC, V3>;
-  else kern = (c.minb >= 3) ? bundle_pc_kernel<WPS, NCH, true, VEC, false> : bundle_pc_kernel<WPS, NCH, false, VEC, false>;
+  else kern = pc_r80(c) ? bundle_pc_kernel<WPS, NCH, true, VEC, false> : bundle_pc_kernel<WPS, NCH, false, VEC, false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem);
   if (e != cudaSuccess) return e;
   if constexpr (V3) {   // the whole point is two 113 KB samples per SM: ask for the largest shared-memory carve-out

@@ -16,6 +16,7 @@
 //   gram pass   : warp owns 4x4 blocks of the k x k output ->  G diag(w) G^T         (shuffle reduce)
 #pragma once
 #include "common.cuh"
+#include "k2_dispatch.cuh"
 
 #include <cooperative_groups.h>
 
@@ -1105,16 +1106,15 @@ __global__ void __launch_bounds__(WPS == 16 ? 512 : 256, MINB) bundle_step_kerne
 
 
 // ---- launch helper shared by the translation units that instantiate the kernel --------------------
-struct K2Config { int wps, cs, nloc, gpitch, npad, ld; size_t smem; };
-
+// (K2Config: k2_dispatch.cuh)
 template <int WPS, int CS>
 static cudaError_t launch_k2(const StepArgs& a, const K2Config& c, int B, cudaStream_t st) {
-  // register budget: 3 CTAs / SM (80 registers) for the small groups and for WPS = 8 when the
-  // shared-memory footprint allows it; the 128-register build otherwise
+  // register budget (c.minb, chosen in bundle_step.cu:k2_fits): 3 CTAs / SM (80 registers) for the small groups and
+  // for WPS = 8 when the shared-memory footprint allows it; the 128-register build otherwise
   void (*kern)(StepArgs);
   if constexpr (WPS == 16) kern = bundle_step_kernel<16, 1, CS>;
   else if constexpr (CS > 1) kern = bundle_step_kernel<WPS, 2, CS>;
-  else if constexpr (WPS == 8) kern = (c.smem * 3 <= 225 * 1024) ? bundle_step_kernel<8, 3, 1> : bundle_step_kernel<8, 2, 1>;
+  else if constexpr (WPS == 8) kern = (c.minb == 3) ? bundle_step_kernel<8, 3, 1> : bundle_step_kernel<8, 2, 1>;
   else kern = bundle_step_kernel<WPS, 3, 1>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem);
   if (e != cudaSuccess) return e;

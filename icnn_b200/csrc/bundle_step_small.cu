@@ -359,7 +359,7 @@ __global__ void __launch_bounds__(128) bundle_step_small_kernel(SmallArgs A) {
   }
 }
 
-bool bundle_step_small_ok(const icnn_bundle_bufs* b) { return b->n <= NM && b->KS <= KM; }
+bool bundle_step_small_ok(int n, int KS) { return n <= NM && KS <= KM; }
 
 int bundle_step_small_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int t, cudaStream_t st) {
   SmallArgs a;

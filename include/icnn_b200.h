@@ -327,6 +327,23 @@ int icnn_tc_set_tuning(int32_t cfg, int32_t splitk, int32_t ch);
 /* out (host, 5 int32) = {tile width BN, ring stages, split-K factor, chunk length, mode} of the calling thread's
  * most recent tensor-core GEMM launch (mode 0 forward, 1 backward, 2 self test, 3 x-path gates; -1 = none yet). */
 int icnn_tc_last_launch(int32_t out[5]);
+/* Which K2 build icnn_bundle_step launches for a problem of n_y = n with KS bundle slots, decided on the host from
+ * the shape, the solver and the launch environment variables (read at every call, as at every launch); nothing is
+ * enqueued and no device is touched.  variant / solver are checked as icnn_bundle_step checks them.  A shape no
+ * build fits returns ICNN_E_UNSUPPORTED with the message the launch would set.  out (host, ICNN_K2_PLAN_LEN int32):
+ *   out[0] kernel family: 0 thread-per-sample (bundle_step_small), 1 two-sweep PC kernel, 2 five-sweep kernel
+ *   out[1] warps per sample (0 for the thread-per-sample kernel)
+ *   out[2] column chunks per thread (two-sweep) or CTAs per cluster (five-sweep; 1 = no cluster); 0 otherwise
+ *   out[3] 1 = two-sweep V3 build (three n-vectors per sample)
+ *   out[4] 1 = 16-byte row loads / tensor-core Gram (n_y % 4 == 0), 0 = scalar row loads / SIMT Gram
+ *   out[5] 1 = bundle rows resident in shared memory (five-sweep ICNN_K2_RESIDENT=1), 0 = streamed from L2
+ *   out[6] minBlocks of the instantiation's __launch_bounds__ (0 = none given)
+ *   out[7] dynamic shared memory per CTA in bytes */
+#define ICNN_K2_PLAN_LEN 8
+int icnn_k2_plan(int32_t n, int32_t KS, int32_t solver, int32_t variant, int32_t out[ICNN_K2_PLAN_LEN]);
+/* out (host, ICNN_K2_PLAN_LEN int32) = the icnn_k2_plan record of the calling thread's most recent K2 enqueue
+ * (icnn_bundle_step, the fused loop or a loop-graph capture); out[0] = -1 and zeros when there was none yet. */
+int icnn_k2_last_launch(int32_t out[ICNN_K2_PLAN_LEN]);
 /* FP64 tensor-core throughput probe: every warp of a full-chip grid issues `iters` x 8 independent
  * mma.m8n8k4.f64 (the instruction K2's weighted-Gram sweep is built from); *flops_out (host) = FLOPs the
  * launch performs, sink (device, 1 double) keeps the result alive.  bench.py times it with CUDA events to

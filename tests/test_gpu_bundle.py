@@ -480,14 +480,36 @@ def test_early_exit_when_all_finished():
 def test_resident_cluster_variant_matches_streaming(name, B, nIter, env, monkeypatch):
     """The optional K2 launch variants (rows resident in shared memory, sample split over a
     thread-block cluster with DSMEM exchanges, 16 warps per sample) compute the same thing as the
-    default streaming kernel.  The launch configuration is read from the environment at every launch."""
-    from icnn_b200 import bundle_entropy as be
+    default streaming kernel.  The launch configuration is read from the environment at every launch.
+    These variables select among five-sweep builds, which the PC solver takes only under ICNN_K2_PC=legacy at these
+    shapes; icnn_k2_last_launch shows that both arms ran the five-sweep kernel and that the variant ran in the second
+    (tests/test_gpu_k2_builds.py compares each variant with the float64 oracle)."""
+    import ctypes as C
+    from icnn_b200 import _capi, bundle_entropy as be
+
+    def ran():
+        out = (C.c_int32 * _capi.K2_PLAN_LEN)()
+        assert _capi.lib.icnn_k2_last_launch(out) == 0
+        return tuple(out)
     p, x, y0 = synth.make_inputs(name, B=B)
     fg = r32(picnn_np.make_fg(p, x))
+    for k_ in ("ICNN_K2_RESIDENT", "ICNN_K2_CS", "ICNN_K2_WPS", "ICNN_K2_SMALL"):
+        monkeypatch.delenv(k_, raising=False)
+    monkeypatch.setenv("ICNN_K2_PC", "legacy")
     ref = be.solveBatch(fg, y0.copy(), nIter=nIter)
+    streaming = ran()
+    assert streaming[0] == 2 and streaming[2] == 1 and streaming[5] == 0, streaming    # five-sweep, no cluster, streamed
     for k_, v_ in env.items():
         monkeypatch.setenv(k_, v_)
     alt = be.solveBatch(fg, y0.copy(), nIter=nIter)
+    variant = ran()
+    assert variant[0] == 2 and variant != streaming, (variant, streaming)
+    if env.get("ICNN_K2_RESIDENT") == "1":
+        assert variant[5] == 1, variant
+    if "ICNN_K2_CS" in env:
+        assert variant[2] == int(env["ICNN_K2_CS"]), variant
+    if "ICNN_K2_WPS" in env:
+        assert variant[1] == int(env["ICNN_K2_WPS"]), variant
     same = (lens(ref[1]) == lens(alt[1])) & (np.array(ref[5]) == np.array(alt[5]))
     assert same.mean() >= 0.8
     assert rowdiff(ref[0], alt[0])[same].max() < 1e-9

@@ -1,7 +1,7 @@
 """Small end-to-end cases for compute-sanitizer (memcheck / racecheck / synccheck):
     compute-sanitizer --tool racecheck python tools/sanitize_case.py
 Covers K1 FFMA + cluster split-K, K1 wgmma path, K2 five-sweep group kernel (1 / 2 / 8 warps per sample, PC + dual +
-RL Newton), every build of the K2 two-sweep PC kernel the dispatch selects, K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the wgmma path (pitch-padded
+RL Newton), every build of the K2 two-sweep PC kernel the dispatch selects, k > 32 bundles and the cluster variant, K2 thread-per-sample kernel, K3, Adam, x-path gates, unaligned widths on the wgmma path (pitch-padded
 operands), GD training backward (FFMA and wgmma GDB instantiation, split-K weight-gradient GEMM)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -18,7 +18,7 @@ def run(name, B, nIter, variant=None, **kw):
     print(name, B, nIter, variant or cfg["variant"], "ok, y range", float(out[0].min()), float(out[0].max()), flush=True)
     return net, fg, out
 
-which = sys.argv[1:] or ["c1", "c3", "c3dual", "c4", "c2", "t", "k3", "adam", "odd", "gdgrad", "pc"]
+which = sys.argv[1:] or ["c1", "c3", "c3dual", "c4", "c2", "t", "k3", "adam", "odd", "gdgrad", "pc", "k2builds"]
 if "c1" in which: run("C1", 16, 4)
 if "c3" in which: run("C3", 6, 4)
 if "c3dual" in which: run("C3", 6, 4, variant="dual")
@@ -65,4 +65,25 @@ if "pc" in which:     # the two-sweep PC kernel in every build bundle_pc.cu sele
     pc_shape(5000, 2, 4)                                # 16 warps / sample, 4 chunks
     _, _, o = run("C3", 4, 4, stats=True)
     print("stats", o[-1].stats()["entering"], flush=True)
+if "k2builds" in which:   # k > 32 in a two-sweep and a five-sweep build, the cluster variant, dual at 16 warps
+    def orthogonal(n, B, P=64):   # one well-separated row per iteration (tests/test_gpu_k2_builds.py)
+        rs = np.random.RandomState(0)
+        P = min(P, n)
+        A = np.zeros((B, P, n))
+        for u in range(B):
+            A[u, np.arange(P), rs.choice(n, P, replace=False)] = 8.0
+        w = rs.randn(n)
+        A = (A + rs.randn(B, P, n) * 0.05 / np.sqrt(n) + 2.0 * w / np.linalg.norm(w)).astype(np.float32).astype(np.float64)
+        b = (0.1 * rs.randn(B, P)).astype(np.float32).astype(np.float64)
+        def fg(y):
+            v = np.einsum("bmn,bn->bm", A, y) + b
+            i = v.argmax(1)
+            return v[np.arange(B), i].astype(np.float32).astype(np.float64), A[np.arange(B), i].copy()
+        return fg
+    for n, nIter, variant, env in ((100, 45, "lib", {}), (100, 62, "lib", {}), (2048, 12, "dual", {"ICNN_K2_CS": "4"}),
+                                   (4096, 40, "dual", {})):
+        os.environ.update(env)
+        out = be.solveBatch(orthogonal(n, 2), np.full((2, n), 0.5), nIter=nIter, variant=variant)
+        for k in env: os.environ.pop(k)
+        print("k2builds n_y", n, nIter, variant, env, "k", [len(g) for g in out[1]], flush=True)
 print("done")
