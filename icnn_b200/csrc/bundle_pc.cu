@@ -24,13 +24,16 @@ ICNN_PC_DECL(1x2_scalar) { return launch_pc<1, 2, false>(a, c, B, st); }
 //   ICNN_PC_V3=0           four-vector 16-warp build at 2048 < n_y <= 4096 (test_three_vector_pc_kernel_matches_four_vector)
 //   ICNN_PC_LEGACY=1       sweep A at rb = 5 as the multi-sweep composition (tests/test_gpu_k2_passes.py)
 //   ICNN_PC_PREFETCH="a,b" L2 prefetch distances of the V3 row sweeps, "0,0" = off (tests/test_gpu_k2_prefetch.py)
-struct PcTestEnv { bool v3, split5; int pfa, pfb; };
+//   ICNN_PC_SEED=0         sweep A at it = 0 and the dependency residual pass always
+//                          (tests/test_gpu_k2_seed.py)
+struct PcTestEnv { bool v3, split5, seed; int pfa, pfb; };
 static PcTestEnv pc_test_env() {
   // prefetch defaults: sweep A one loop trip ahead, sweep B eight rows ahead (chosen per setting with
   // tools/k2_profile.py at C5 on H100, DESIGN.md §3 "Row passes")
-  PcTestEnv e = {true, false, 1, 8};
+  PcTestEnv e = {true, false, true, 1, 8};
   if (const char* v = getenv("ICNN_PC_V3")) e.v3 = v[0] != '0';
   if (const char* v = getenv("ICNN_PC_LEGACY")) e.split5 = v[0] == '1';
+  if (const char* v = getenv("ICNN_PC_SEED")) e.seed = v[0] != '0';
   if (const char* v = getenv("ICNN_PC_PREFETCH")) {
     int pa = 0, pb = 0;
     if (sscanf(v, "%d,%d", &pa, &pb) == 2 && pa >= 0 && pa <= 8 && pb >= 0 && pb <= 64) { e.pfa = pa; e.pfb = pb; }
@@ -85,7 +88,7 @@ int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int 
   const PcTestEnv env = pc_test_env();
   PcArgs a;
   a.b = *b; a.c = *cfg; a.t = t; a.npad = c.npad;
-  a.split5 = env.split5; a.pfa = env.pfa; a.pfb = env.pfb;
+  a.split5 = env.split5; a.seed = env.seed; a.pfa = env.pfa; a.pfb = env.pfb;
   cudaError_t e;
   if (c.v3) e = launch_pc_v3_8x4(a, c, b->B, st);
   else if (c.wps == 16) e = c.nch == 2 ? launch_pc_16x2(a, c, b->B, st) : launch_pc_16x4(a, c, b->B, st);

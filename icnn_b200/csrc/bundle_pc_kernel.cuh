@@ -19,9 +19,12 @@
 //
 // Passes over a sample's k bundle rows per outer iteration (at n_y = 4096 a row is 16 KB and the rows of the resident
 // samples do not fit in L2, so each pass is mostly HBM traffic):
-//   append (Gram row + duplicate flags) 1; dependency test 1 residual pass, + 1 dot pass and 1 more residual pass when
-//   it refines; u0 = G^T z0 1; per interior-point iteration: sweep A 1 (rb = ceil((k + 2) / 8) <= 4; V3 also rb = 5,
-//   see gram_pass_pc) and sweep B 1.  ~8 interior-point iterations at C5 -> about 2 its + 3 passes.
+//   append (Gram row + duplicate flags) 1; dependency test: none when the last pivot of the bordered Cholesky of the
+//   Gram says "clearly independent", else 1 residual pass, + 1 dot pass and 1 more residual pass when it refines;
+//   u0 = G^T z0 1; per interior-point iteration: sweep A 1 (rb = ceil((k + 2) / 8) <= 4; V3 also rb = 5, see
+//   gram_pass_pc) except at it = 0, whose M0, q, w follow from the stored unweighted Gram, and sweep B 1; sweep A also
+//   runs in the iteration that only detects convergence.  its interior-point steps (~8 at C5) -> 2 its + 2 passes in
+//   the common case.
 //
 // Shared memory per sample: 4 n-vectors (y, u, ry|du, v1+v3|dy), ONE packed lower-triangular k x k matrix,
 // 18 k-vectors.  All reductions over n_y and all k x k algebra are FP64, as in the reference.
@@ -46,6 +49,8 @@ struct PcArgs {
   int pfa;   // V3 sweep A: L2 prefetch of the row groups this many loop trips ahead (0 = none)
   int pfb;   // V3 sweep B: L2 prefetch of the row this many rows ahead (0 = none)
   bool split5;  // sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY=1, see gram_pass_pc)
+  bool seed;    // interior-point iteration 0 from the stored Gram, dependency residual pass only when needed
+                // (false: ICNN_PC_SEED=0, both passes always)
 };
 
 // L2 prefetch of the line holding p (no register is held for it and no result comes back: it only starts the HBM read
@@ -108,10 +113,11 @@ __device__ inline bool warp_cholesky_p(double* L, double* invd, int k, int lane)
   return k <= 32 ? warp_cholesky_impl<true>(L, invd, k, lane) : warp_cholesky_impl<false>(L, invd, k, lane);
 }
 
-// L L^T X = B for NR right-hand sides held in registers (lane r owns rows r, r + 32), pivots by shuffle.
+// L X = B (forward substitution) for NR right-hand sides held in registers (lane r owns rows r, r + 32), pivots by
+// shuffle.
 template <int NR, bool K32>
-__device__ __forceinline__ void warp_chol_solve_impl(const double* L, const double* invd, int k, double (&b0)[NR],
-                                                     double (&b1)[NR], int lane) {
+__device__ __forceinline__ void warp_chol_fwd_impl(const double* L, const double* invd, int k, double (&b0)[NR],
+                                                   double (&b1)[NR], int lane) {
   const int r0 = lane, r1 = lane + 32;
   const int o0 = lidx(r0, 0), o1 = lidx(r1, 0);
   for (int i = 0; i < k; ++i) {
@@ -125,6 +131,12 @@ __device__ __forceinline__ void warp_chol_solve_impl(const double* L, const doub
       if (!K32) b1[q] = (r1 == i) ? xi : fma(-l1, xi, b1[q]);
     }
   }
+}
+// L^T X = B (backward substitution)
+template <int NR, bool K32>
+__device__ __forceinline__ void warp_chol_bwd_impl(const double* L, const double* invd, int k, double (&b0)[NR],
+                                                   double (&b1)[NR], int lane) {
+  const int r0 = lane, r1 = lane + 32;
   for (int i = k - 1; i >= 0; --i) {
     const double di = invd[i];
     const int oi = lidx(i, 0);
@@ -138,11 +150,35 @@ __device__ __forceinline__ void warp_chol_solve_impl(const double* L, const doub
     }
   }
 }
+// L L^T X = B
+template <int NR, bool K32>
+__device__ __forceinline__ void warp_chol_solve_impl(const double* L, const double* invd, int k, double (&b0)[NR],
+                                                     double (&b1)[NR], int lane) {
+  warp_chol_fwd_impl<NR, K32>(L, invd, k, b0, b1, lane);
+  warp_chol_bwd_impl<NR, K32>(L, invd, k, b0, b1, lane);
+}
 template <int NR>
 __device__ inline void warp_chol_solve_p(const double* L, const double* invd, int k, double (&b0)[NR],
                                          double (&b1)[NR], int lane) {
   if (k <= 32) warp_chol_solve_impl<NR, true>(L, invd, k, b0, b1, lane);
   else warp_chol_solve_impl<NR, false>(L, invd, k, b0, b1, lane);
+}
+// L L^T x = b for one right-hand side; also returns |L^-1 b|^2 (the forward solve's sum of squares, every lane).  With L
+// the Cholesky factor of the Gram of k rows and b their dot products with one more row r, |r|^2 - |L^-1 b|^2 is the last
+// pivot of the bordered factor: the squared distance of r from the span of the k rows, backward stable.
+template <bool K32>
+__device__ __forceinline__ double warp_chol_solve_fwdsq_impl(const double* L, const double* invd, int k, double (&b0)[1],
+                                                             double (&b1)[1], int lane) {
+  warp_chol_fwd_impl<1, K32>(L, invd, k, b0, b1, lane);
+  const double f0 = lane < k ? b0[0] : 0.0, f1 = (!K32 && lane + 32 < k) ? b1[0] : 0.0;
+  const double fs = Grp<1>::wsum(fma(f0, f0, f1 * f1));
+  warp_chol_bwd_impl<1, K32>(L, invd, k, b0, b1, lane);
+  return fs;
+}
+__device__ inline double warp_chol_solve_fwdsq_p(const double* L, const double* invd, int k, double (&b0)[1],
+                                                 double (&b1)[1], int lane) {
+  return k <= 32 ? warp_chol_solve_fwdsq_impl<true>(L, invd, k, b0, b1, lane)
+                 : warp_chol_solve_fwdsq_impl<false>(L, invd, k, b0, b1, lane);
 }
 
 // get_step (lib/bundle_entropy.py:158-163) over a k-vector whose elements j = lane, lane + 32 sit in registers
@@ -630,22 +666,27 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
         for (int j = 0; j <= i; ++j) Lp[lidx(i, j)] = gramu[(size_t)permu[i] * KS + permu[j]];
       __syncwarp();
       const bool ok = warp_cholesky_p(Lp, invd, k0, g.lane);
+      double fs = 0.0;
       if (ok) {
         double b0[1] = {g.lane < k0 ? tk[g.lane] : 0.0}, b1[1] = {g.lane + 32 < k0 ? tk[g.lane + 32] : 0.0};
-        warp_chol_solve_p<1>(Lp, invd, k0, b0, b1, g.lane);
+        fs = warp_chol_solve_fwdsq_p(Lp, invd, k0, b0, b1, g.lane);
         if (g.lane < k0) rk[g.lane] = b0[0];
         if (g.lane + 32 < k0) rk[g.lane + 32] = b1[0];
       }
       double md = tk[k0];
       for (int j = g.lane; j < k0; j += 32) md = fmax(md, gramu[(size_t)permu[j] * KS + permu[j]]);
       md = Grp<1>::wmax(md);
-      if (g.lane == 0) { isc[1] = ok ? 1 : 0; sc[9] = md; }
+      // Clearly independent: the squared distance of the new row from the span, tk[k0] - |L^-1 tk|^2 (error ~ k eps
+      // maxdiag), is 100x above both thresholds of the residual pass below, which could then only conclude
+      // "independent": that pass is skipped.
+      const bool clear = A.seed && ok && tk[k0] - fs > 100.0 * fmax(cf.rank_tol * cf.rank_tol * md, 1e-8 * md);
+      if (g.lane == 0) { isc[1] = ok ? 1 : 0; isc[4] = clear ? 1 : 0; sc[9] = md; }
       __syncwarp();
     }
     g.sync();
     const double maxdiag = sc[9];
     if (isc[0]) dependent = true;
-    else if (!isc[1]) dependent = false;
+    else if (!isc[1] || isc[4]) dependent = false;
     else {
       const double thr2 = cf.rank_tol * cf.rank_tol * maxdiag;
       for (int rep = 0; rep < 2; ++rep) {
@@ -690,15 +731,42 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     PCKV(3)[j] = 1.0;       // s
   }
   if (g.tid == 0) sc[0] = 1.0;  // t
-  // pads of the n-vectors the tensor-core sweep reads: y = 0.5, ry = 0 (finite; the G loads there are zero)
-  for (int e = n + g.tid; e < npad; e += T) { yv[e] = 0.5; rv[e] = 0.0; }
+  // y = 0.5 (logit = 0); pads of the n-vectors the tensor-core sweep reads: ry = 0 (finite; the G loads there are zero)
+  for (int e = g.tid; e < npad; e += T) { yv[e] = 0.5; if (e >= n) rv[e] = 0.0; }
   g.sync();
 
   // =====================  Mehrotra predictor-corrector, lib/bundle_entropy.py:5-78  =====================
   const int maxit = cf.max_inner > 0 ? cf.max_inner : 20;
   int inner_its = 0, fail = 0;
   int zsel = 0;   // z lives in k-vector 1 + zsel, s in 3 + zsel; the update writes the other buffer
-  // y = 0.5 (logit = 0), u = G^T z0, ry = u
+  const int j0 = g.lane, j1 = g.lane + 32;
+  const bool v0 = j0 < k, v1ok = j1 < k;
+  // Seeded iteration 0: the start y = 0.5, z = z0 = 1/k, s = 1, t = 1 gives D = 0.25 exactly, so M0 = 0.25 G G^T,
+  // w = G y = 0.5 rowsum and q = G (D o G^T z0) = M0 z0 follow from the unweighted Gram and row sums kept in b.gram /
+  // b.rsum (the same sums in another FP64 order): no sweep A at it = 0.  A sample whose seeded dr is below 1e-6 (the
+  // stopping test wants sqrt(dr) < 1e-8, so the rounding of the seeded w could decide it) takes sweep A at it = 0.
+  bool seed0 = false;
+  if (A.seed) {
+    for (int p = g.tid; p < k * k; p += T) {
+      const int i = p / k, j = p - i * k;
+      if (j <= i) Lp[lidx(i, j)] = 0.25 * gramu[(size_t)permu[i] * KS + permu[j]];
+    }
+    g.sync();
+    for (int i = g.tid; i < k; i += T) {
+      const double* z = PCKV(1);
+      double q = 0.0;
+      for (int j = 0; j < k; ++j) q = fma(j <= i ? Lp[lidx(i, j)] : Lp[lidx(j, i)], z[j], q);
+      qk[i] = q;
+      wk[i] = 0.5 * rsu[permu[i]];
+    }
+    g.sync();
+    // rd and dr as pc_kxk_stage forms them at it = 0 (every warp, redundantly)
+    const double rd0 = v0 ? ((wk[j0] + hk[j0]) - sc[0]) + PCKV(3)[j0] : 0.0;
+    const double rd1 = v1ok ? ((wk[j1] + hk[j1]) - sc[0]) + PCKV(3)[j1] : 0.0;
+    const double dr = Grp<1>::wsum(fma(rd0, rd0, rd1 * rd1));
+    seed0 = sqrt(dr) >= 1e-6;
+  }
+  // u = G^T z0, ry = u
   double pr = 0.0;
   {
     const double* const w1r[1] = {PCKV(1)};
@@ -711,19 +779,18 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         const int e = pc_col<T, VEC>(cb, g.tid, c);
-        if (e < n) { yv[e] = 0.5; if (!V3) uv[e] = acc[0][c]; rv[e] = acc[0][c]; pr = fma(acc[0][c], acc[0][c], pr); }
+        if (e < n) { if (!V3) uv[e] = acc[0][c]; rv[e] = acc[0][c]; pr = fma(acc[0][c], acc[0][c], pr); }
       }
     }
   }
   pr = red.sum(g, pr);
-  const int j0 = g.lane, j1 = g.lane + 32;
-  const bool v0 = j0 < k, v1ok = j1 < k;
 #pragma unroll 1
   for (int it = 0; it < maxit; ++it) {
     double* zc = PCKV(1 + zsel);
     double* scur = PCKV(3 + zsel);
+    const bool seeded = seed0 && it == 0;   // M0, q, w in place
     // ---- sweep A (warp 0 ends up holding M0, q, w in shared memory)
-    gram_pass_pc<WPS, VEC, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, A.split5, V3 ? A.pfa : 0);
+    if (!seeded) gram_pass_pc<WPS, VEC, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, A.split5, V3 ? A.pfa : 0);
     // ---- k x k stage
     if (g.warp == 0) {
       const PcKxk io{Lp, invd, zc, scur, wk, hk, qk, dza, dzp, dzq, dsa, sc, isc};

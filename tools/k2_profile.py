@@ -10,7 +10,10 @@ environment knobs that bundle_pc.cu reads at every launch, so all builds run in 
 Per t it prints the ms of the K2 launch for each build, the mean active rows k of a solve, the mean interior-point
 iterations, and the modelled row bytes over the time of the first build:
     sum over the samples of passes x k x n x 4,  passes = 2 its + PASSES_OUTSIDE
-(sweeps A and B per interior-point iteration, plus the passes outside the interior-point loop)."""
+with its the interior-point steps of a solve: sweep B once per step, sweep A once per step counting the iteration that
+only detects convergence but not the seeded iteration 0, and PASSES_OUTSIDE = 2 for the append pass and u0 = G^T z0.
+The dependency test's residual pass (skipped when the new row is clearly independent) is not modelled; for the
+seed0 build (ICNN_PC_SEED=0, sweep A at it = 0 and the residual pass always) set K2_PASSES_OUTSIDE=4."""
 import argparse
 import ctypes as C
 import json
@@ -25,6 +28,7 @@ BUILDS = {
     "v3": {},                      # the default at 2048 < n_y <= 4096
     "v3off": {"ICNN_PC_V3": "0"},  # 16-warp four-vector kernel, one sample per SM
     "legacy": {"ICNN_PC_LEGACY": "1"},
+    "seed0": {"ICNN_PC_SEED": "0"},  # sweep A at it = 0 and the dependency residual pass always
     # L2 prefetch distances of the V3 row sweeps, "sweep A trips,sweep B rows" (bundle_pc.cu)
     "pf0": {"ICNN_PC_PREFETCH": "0,0"},
     "pfa1": {"ICNN_PC_PREFETCH": "1,0"},
@@ -35,7 +39,7 @@ BUILDS = {
     "pfa2b16": {"ICNN_PC_PREFETCH": "2,16"},
 }
 KNOBS = sorted({k for e in BUILDS.values() for k in e})
-PASSES_OUTSIDE = int(os.environ.get("K2_PASSES_OUTSIDE", "5"))
+PASSES_OUTSIDE = int(os.environ.get("K2_PASSES_OUTSIDE", "2"))
 
 
 def main():
