@@ -26,14 +26,17 @@ ICNN_PC_DECL(1x2_scalar) { return launch_pc<1, 2, false>(a, c, B, st); }
 //   ICNN_PC_PREFETCH="a,b" L2 prefetch distances of the V3 row sweeps, "0,0" = off (tests/test_gpu_k2_prefetch.py)
 //   ICNN_PC_SEED=0         sweep A at it = 0 and the dependency residual pass always
 //                          (tests/test_gpu_k2_seed.py)
-struct PcTestEnv { bool v3, split5, seed; int pfa, pfb; };
+//   ICNN_PC_TWOLOG=1       V3 update with two logs, ry_new = logit(y_new) + (ry_old - logit(y_old)) + a du
+//                          (tests/test_gpu_k2_onelog.py)
+struct PcTestEnv { bool v3, split5, seed, twolog; int pfa, pfb; };
 static PcTestEnv pc_test_env() {
   // prefetch defaults: sweep A one loop trip ahead, sweep B eight rows ahead (chosen per setting with
   // tools/k2_profile.py at C5 on H100, DESIGN.md §3 "Row passes")
-  PcTestEnv e = {true, false, true, 1, 8};
+  PcTestEnv e = {true, false, true, false, 1, 8};
   if (const char* v = getenv("ICNN_PC_V3")) e.v3 = v[0] != '0';
   if (const char* v = getenv("ICNN_PC_LEGACY")) e.split5 = v[0] == '1';
   if (const char* v = getenv("ICNN_PC_SEED")) e.seed = v[0] != '0';
+  if (const char* v = getenv("ICNN_PC_TWOLOG")) e.twolog = v[0] == '1';
   if (const char* v = getenv("ICNN_PC_PREFETCH")) {
     int pa = 0, pb = 0;
     if (sscanf(v, "%d,%d", &pa, &pb) == 2 && pa >= 0 && pa <= 8 && pb >= 0 && pb <= 64) { e.pfa = pa; e.pfb = pb; }
@@ -88,7 +91,7 @@ int bundle_pc_launch(const icnn_bundle_cfg* cfg, const icnn_bundle_bufs* b, int 
   const PcTestEnv env = pc_test_env();
   PcArgs a;
   a.b = *b; a.c = *cfg; a.t = t; a.npad = c.npad;
-  a.split5 = env.split5; a.seed = env.seed; a.pfa = env.pfa; a.pfb = env.pfb;
+  a.split5 = env.split5; a.seed = env.seed; a.twolog = env.twolog; a.pfa = env.pfa; a.pfb = env.pfb;
   cudaError_t e;
   if (c.v3) e = launch_pc_v3_8x4(a, c, b->B, st);
   else if (c.wps == 16) e = c.nch == 2 ? launch_pc_16x2(a, c, b->B, st) : launch_pc_16x4(a, c, b->B, st);

@@ -33,9 +33,11 @@
 // (n_y = 4096: 128 KB) the kernel is latency-bound on that one sample's serial stages (the one-warp k x k
 // factor/solves, the tree sums); with three vectors and 12 aliased k-vectors a sample needs <= 113 KB, so TWO
 // 8-warp samples are resident per SM and one sample's serial stage overlaps the other's sweeps.  u = G^T z is
-// not stored: u_old = ry_old - logit(y_old) is recovered in the update (one more log per element per
-// interior-point iteration), and dy = -D (ry + du) is recomputed there from the stored du (same expression,
-// same inputs -> the same bits as the value the step bound was taken from).
+// not stored: the update forms ry_new = logit(y_new) + u_old + a du with u_old = ry_old - logit(y_old), as
+// ry_old + a du + log(y_new (1 - y_old) / (y_old (1 - y_new))) (one log and one division per element), and
+// dy = -D (ry + du) is recomputed there from the stored du (same expression, same inputs -> the same bits as the
+// value the step bound was taken from).  The V3 n-vectors are stored
+// thread-interleaved (pc_pos), so the per-element phases access shared memory without bank conflicts.
 #pragma once
 #include "bundle_step_kernel.cuh"
 
@@ -51,7 +53,46 @@ struct PcArgs {
   bool split5;  // sweep A at rb = 5 as the multi-sweep composition (ICNN_PC_LEGACY=1, see gram_pass_pc)
   bool seed;    // interior-point iteration 0 from the stored Gram, dependency residual pass only when needed
                 // (false: ICNN_PC_SEED=0, both passes always)
+  bool twolog;  // V3 update: ry_new = logit(y_new) + (ry_old - logit(y_old)) + a du, two logs (ICNN_PC_TWOLOG=1);
+                // false: ry_old + a du + log(y_new (1 - y_old) / (y_old (1 - y_new))), one log
+#ifdef ICNN_PC_PHASES
+  unsigned long long* ph;   // [t][PC_NPH][PC_PH_SLOTS] clock64 cycles (tools/k2_phases.py)
+#endif
 };
+
+// Phase timers (tools/k2_phases.py builds the kernel with ICNN_PC_PHASES into a shared object of its own; the library
+// never has them): thread 0 of each CTA reads clock64 at the end of each phase and adds the cycles since the previous
+// mark to the phase's counter of outer iteration t, spread over PC_PH_SLOTS addresses by CTA.  Thread 0 is in warp 0,
+// so a phase that ends at a barrier includes the wait for the slowest warp.
+enum PcPhase {
+  PC_PH_APPEND = 0,   // append, dependency test, z / s / pads of the start point
+  PC_PH_SEED,         // seeded M0, q, w of iteration 0
+  PC_PH_U0,           // u0 = G^T z0 and its reduction
+  PC_PH_SWEEPA,       // sweep A with its tree sum
+  PC_PH_KXK,          // k x k stage (warp 0) and the barrier after it
+  PC_PH_SWEEPB,       // sweep B with its step-bound reduction
+  PC_PH_SIGMA,        // sigma and the combined k-space direction
+  PC_PH_DIR2,         // second direction pass with its reduction, z / s update
+  PC_PH_UPDATE,       // y, ry update with its reduction
+  PC_PH_COMMIT,       // commit y, lambda, prune
+  PC_NPH
+};
+constexpr int PC_PH_SLOTS = 32;
+#ifdef ICNN_PC_PHASES
+#define PC_PHASE_START() long long pc_ph_t = clock64()
+#define PC_PHASE(i)                                                                                              \
+  do {                                                                                                           \
+    if (threadIdx.x == 0) {                                                                                      \
+      const long long pc_c = clock64();                                                                          \
+      atomicAdd(A.ph + ((size_t)A.t * PC_NPH + (i)) * PC_PH_SLOTS + (blockIdx.x & (PC_PH_SLOTS - 1)),            \
+                (unsigned long long)(pc_c - pc_ph_t));                                                           \
+      pc_ph_t = pc_c;                                                                                            \
+    }                                                                                                            \
+  } while (0)
+#else
+#define PC_PHASE_START() do {} while (0)
+#define PC_PHASE(i) do {} while (0)
+#endif
 
 // L2 prefetch of the line holding p (no register is held for it and no result comes back: it only starts the HBM read
 // early).  Used by the row sweeps of the V3 kernel, which are bound by the latency of their row loads.
@@ -230,6 +271,21 @@ struct PcRed {
 // D = y (1 - y) = 1 / (1/y + 1/(1-y))  (lib/bundle_entropy.py:18), one FMA; the same expression everywhere
 __device__ __forceinline__ double dweight(double y) { return fma(-y, y, y); }
 
+// ---- where n-vector element e sits in shared memory -----------------------------------------------------------------
+// IL (V3 build): thread-interleaved.  The per-element phases give thread tid the columns e = cb + 4 tid + c (c < 4) of
+// each chunk cb of 4 T columns (one 128-bit row load per row); element e sits at cb + c tc + tid, with tc = T, or a
+// quarter of the last chunk when that one is partial (npad - cb < 4 T; npad is a multiple of 16).  A warp's access in
+// those phases is then 32 consecutive doubles (2 wavefronts) instead of doubles 32 bytes apart (a 4-way bank conflict).
+// Not IL: element e at e.
+template <int T, bool IL>
+__device__ __forceinline__ int pc_tc(int cb, int npad) { return IL ? ::min(T, (npad - cb) >> 2) : 1; }
+template <int T, bool IL>
+__device__ __forceinline__ int pc_pos(int e, int npad) {
+  if (!IL) return e;
+  const int cb = e & ~(4 * T - 1);
+  return cb + (e & 3) * pc_tc<T, IL>(cb, npad) + ((e - cb) >> 2);
+}
+
 // ---- sweep A: weighted Gram + the two pseudo-rows on the FP64 tensor cores --------------------------
 // Sweep rows: R = 0 -> pseudo-row whose A-fragment value is D_j ry_j  (result row 0:  q = G (D o ry)),
 //             R = 1 -> pseudo-row whose A-fragment value is y_j       (result row 1:  w = G y),
@@ -239,8 +295,9 @@ __device__ __forceinline__ double dweight(double y) { return fma(-y, y, y); }
 // elements for four consecutive k-steps.  The n-vectors are padded to a multiple of 16 doubles with finite
 // values, so only the loads of G are predicated.  The warp partials are summed by a fixed tree through a
 // scratch n-vector (deterministic), and warp 0 stores the result (packed matrix / q / w).
-// VEC: rows are 16-byte aligned (n % 4 == 0) -> one 128-bit load per row block.
-template <int WPS, int NA, int NB, bool TRI, bool PSEUDO, bool VEC, class G>
+// VEC: rows are 16-byte aligned (n % 4 == 0) -> one 128-bit load per row block.  IL (V3 build): y and ry in the
+// interleaved layout (pc_pos); scap, the scratch vector's doubles, is then npad.
+template <int WPS, int NA, int NB, bool TRI, bool PSEUDO, bool VEC, bool IL, class G>
 __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                               const double* rv, double* Lp, double* qk, double* wk, double* scratch,
                                               int scap, int a0, int b0, int pfd = 0) {
@@ -305,17 +362,37 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
       const int gu = gi + u * WPS;
       if (u > 0 && gu >= ngrp) break;
       const int off = gu * 16;
-      const double2 ya = *reinterpret_cast<const double2*>(yq + off);
-      const double2 yb = *reinterpret_cast<const double2*>(yq + off + 2);
-      double dd[4] = {dweight(ya.x), dweight(ya.y), dweight(yb.x), dweight(yb.y)};
+      double ys[4];
+      int p0 = 0, tc = 0;   // IL: elements off + 4q + s at p0 + s tc
+      if (IL) {
+        const int e0 = off + 4 * q, cb = e0 & ~(4 * 32 * WPS - 1);
+        tc = pc_tc<32 * WPS, true>(cb, scap);
+        p0 = cb + ((e0 - cb) >> 2);
+#pragma unroll
+        for (int s = 0; s < 4; ++s) ys[s] = yv[p0 + s * tc];
+      } else {
+        const double2 ya = *reinterpret_cast<const double2*>(yq + off);
+        const double2 yb = *reinterpret_cast<const double2*>(yq + off + 2);
+        ys[0] = ya.x; ys[1] = ya.y; ys[2] = yb.x; ys[3] = yb.y;
+      }
+      double dd[4] = {dweight(ys[0]), dweight(ys[1]), dweight(ys[2]), dweight(ys[3])};
       double pa[4] = {0.0, 0.0, 0.0, 0.0};
       if (PSEUDO && ps) {
         if (r == 0) {
-          const double2 ra = *reinterpret_cast<const double2*>(rq + off);
-          const double2 rb = *reinterpret_cast<const double2*>(rq + off + 2);
-          pa[0] = dd[0] * ra.x; pa[1] = dd[1] * ra.y; pa[2] = dd[2] * rb.x; pa[3] = dd[3] * rb.y;
+          double rs[4];
+          if (IL) {
+#pragma unroll
+            for (int s = 0; s < 4; ++s) rs[s] = rv[p0 + s * tc];
+          } else {
+            const double2 ra = *reinterpret_cast<const double2*>(rq + off);
+            const double2 rb = *reinterpret_cast<const double2*>(rq + off + 2);
+            rs[0] = ra.x; rs[1] = ra.y; rs[2] = rb.x; rs[3] = rb.y;
+          }
+#pragma unroll
+          for (int s = 0; s < 4; ++s) pa[s] = dd[s] * rs[s];
         } else {
-          pa[0] = ya.x; pa[1] = ya.y; pa[2] = yb.x; pa[3] = yb.y;
+#pragma unroll
+          for (int s = 0; s < 4; ++s) pa[s] = ys[s];
         }
       }
 #pragma unroll
@@ -407,12 +484,12 @@ __device__ __forceinline__ void gram_sweep_pc(const G& g, const float* const* ro
   }
 }
 
-template <int WPS, int NB, bool VEC, class G>
+template <int WPS, int NB, bool VEC, bool IL, class G>
 __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                                   const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
                                                   int pfd) {
-  gram_sweep_pc<WPS, 2, NB, false, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4, pfd);
-  gram_sweep_pc<WPS, 2, NB, false, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4, pfd);
+  gram_sweep_pc<WPS, 2, NB, false, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 4, pfd);
+  gram_sweep_pc<WPS, 2, NB, false, false, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 2, 4, pfd);
 }
 
 // k + 2 sweep rows in rb = ceil((k + 2) / 8) <= 8 row blocks (k <= 62).  On return warp 0 has stored M0, q, w.
@@ -421,24 +498,24 @@ __device__ __forceinline__ void gram_rect_pair_pc(const G& g, const float* const
 // accumulators in one sweep would spill).  ONE5 (V3 build only: the other builds have no register room for 15 tiles)
 // enables the one-sweep rb = 5, which at C5 carries the last outer iterations (k = 31..38); split5 sends rb = 5 through
 // the composition anyway (11 block loads instead of 5; ICNN_PC_LEGACY=1, the form the one sweep is tested against).
-template <int WPS, bool VEC, bool ONE5, class G>
+template <int WPS, bool VEC, bool ONE5, bool IL, class G>
 __device__ __forceinline__ void gram_pass_pc(const G& g, const float* const* rowp, int k, int n, const double* yv,
                                              const double* rv, double* Lp, double* qk, double* wk, double* sx, int scap,
                                              bool split5, int pfd) {
   const int rb = (k + 2 + 7) >> 3;
-  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
-  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
-  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  if (rb == 1) gram_sweep_pc<WPS, 1, 1, true, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 2) gram_sweep_pc<WPS, 2, 2, true, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+  else if (rb == 3) gram_sweep_pc<WPS, 3, 3, true, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   else if (ONE5 && rb == 5 && !split5) {
-    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+    if constexpr (ONE5) gram_sweep_pc<WPS, 5, 5, true, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
   } else {
-    gram_sweep_pc<WPS, 4, 4, true, true, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
+    gram_sweep_pc<WPS, 4, 4, true, true, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 0, 0, pfd);
     if (rb > 4) {
       const int r2 = rb - 4;
-      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 1, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 2, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 3, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
-      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 4, VEC>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      if (r2 == 1) { gram_sweep_pc<WPS, 1, 1, true, false, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 1, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 2) { gram_sweep_pc<WPS, 2, 2, true, false, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 2, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else if (r2 == 3) { gram_sweep_pc<WPS, 3, 3, true, false, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 3, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
+      else { gram_sweep_pc<WPS, 4, 4, true, false, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, 4, 4, pfd); gram_rect_pair_pc<WPS, 4, VEC, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, sx, scap, pfd); }
     }
   }
 }
@@ -564,7 +641,10 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   if (u >= b.B) return;
   if (b.finished[u]) return;
 
+  PC_PHASE_START();
   const int n = b.n, KS = b.KS, npad = A.npad;
+  constexpr bool IL = V3;   // interleaved n-vectors (pc_pos)
+  static_assert(!IL || VEC, "IL");
   double* base = smem_d + (size_t)g.gid * pc_group_doubles(npad, KS, WPS, V3);
   double* yv = base;
   double* uv = V3 ? nullptr : yv + npad;   // V3: u is not stored (recovered as ry - logit(y) in the update)
@@ -633,6 +713,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     if (g.tid == 0) { stat_add(b.iter_stats, A.t, 0, 1.0); stat_add(b.iter_stats, A.t, 6, fu + ent); }
     if (bad > 0.0 || !isfinite(fu)) {
       if (g.tid == 0) { b.status[u] = ICNN_ST_NONFINITE; b.finished[u] = 1; b.nIters[u] = A.t - 1; stat_add(b.iter_stats, A.t, 5, 1.0); }
+      PC_PHASE(PC_PH_APPEND);
       return;
     }
     for (int j = g.warp; j < k; j += WPS) {
@@ -721,6 +802,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   }
   if (dependent) {
     if (g.tid == 0) { b.status[u] = ICNN_ST_RANK_STOP; b.finished[u] = 1; b.nIters[u] = A.t - 1; stat_add(b.iter_stats, A.t, 5, 1.0); }
+    PC_PHASE(PC_PH_APPEND);
     return;
   }
   for (int j = g.tid; j < k; j += T) {
@@ -732,8 +814,9 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   }
   if (g.tid == 0) sc[0] = 1.0;  // t
   // y = 0.5 (logit = 0); pads of the n-vectors the tensor-core sweep reads: ry = 0 (finite; the G loads there are zero)
-  for (int e = g.tid; e < npad; e += T) { yv[e] = 0.5; if (e >= n) rv[e] = 0.0; }
+  for (int e = g.tid; e < npad; e += T) { yv[e] = 0.5; if (e >= n) rv[pc_pos<T, IL>(e, npad)] = 0.0; }
   g.sync();
+  PC_PHASE(PC_PH_APPEND);
 
   // =====================  Mehrotra predictor-corrector, lib/bundle_entropy.py:5-78  =====================
   const int maxit = cf.max_inner > 0 ? cf.max_inner : 20;
@@ -766,6 +849,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     const double dr = Grp<1>::wsum(fma(rd0, rd0, rd1 * rd1));
     seed0 = sqrt(dr) >= 1e-6;
   }
+  PC_PHASE(PC_PH_SEED);
   // u = G^T z0, ry = u
   double pr = 0.0;
   {
@@ -774,23 +858,27 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     for (int ch = 0; ch < NCH; ++ch) {
       const int cb = ch * 4 * T;
       if (cb >= n) break;
+      const int tc = pc_tc<T, IL>(cb, npad);
       double acc[1][4];
       col_dots_pc<T, 1, VEC>(rowp, k, n, cb, g.tid, w1r, acc);
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         const int e = pc_col<T, VEC>(cb, g.tid, c);
-        if (e < n) { if (!V3) uv[e] = acc[0][c]; rv[e] = acc[0][c]; pr = fma(acc[0][c], acc[0][c], pr); }
+        const int pe = IL ? cb + c * tc + g.tid : e;
+        if (e < n) { if (!V3) uv[pe] = acc[0][c]; rv[pe] = acc[0][c]; pr = fma(acc[0][c], acc[0][c], pr); }
       }
     }
   }
   pr = red.sum(g, pr);
+  PC_PHASE(PC_PH_U0);
 #pragma unroll 1
   for (int it = 0; it < maxit; ++it) {
     double* zc = PCKV(1 + zsel);
     double* scur = PCKV(3 + zsel);
     const bool seeded = seed0 && it == 0;   // M0, q, w in place
     // ---- sweep A (warp 0 ends up holding M0, q, w in shared memory)
-    if (!seeded) gram_pass_pc<WPS, VEC, V3>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, A.split5, V3 ? A.pfa : 0);
+    if (!seeded) gram_pass_pc<WPS, VEC, V3, IL>(g, rowp, k, n, yv, rv, Lp, qk, wk, xv, npad, A.split5, V3 ? A.pfa : 0);
+    PC_PHASE(PC_PH_SWEEPA);
     // ---- k x k stage
     if (g.warp == 0) {
       const PcKxk io{Lp, invd, zc, scur, wk, hk, qk, dza, dzp, dzq, dsa, sc, isc};
@@ -798,6 +886,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       else pc_kxk_stage<false>(io, k, g.lane, pr);
     }
     g.sync();
+    PC_PHASE(PC_PH_KXK);
     if (isc[2]) break;
     if (isc[3]) { fail = 1; break; }
     inner_its = it + 1;
@@ -810,17 +899,19 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       for (int ch = 0; ch < NCH; ++ch) {
         const int cb = ch * 4 * T;
         if (cb >= n) break;
+        const int tc = pc_tc<T, IL>(cb, npad);
         double acc[3][4];
         col_dots_pc<T, 3, VEC, V3 ? 8 : 4>(rowp, k, n, cb, g.tid, w3, acc, V3 ? A.pfb : 0);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const int e = pc_col<T, VEC>(cb, g.tid, c);
+          const int pe = IL ? cb + c * tc + g.tid : e;
           if (e < n) {
-            const double ye = yv[e];
-            const double dy = -dweight(ye) * (rv[e] + acc[0][c]);
+            const double ye = yv[pe];
+            const double dy = -dweight(ye) * (rv[pe] + acc[0][c]);
             if (dy < 0.0) ratio_min(n1, d1, ye, -dy);          // get_step(y, dy)
             if (dy > 0.0) ratio_min(n2, d2, 1.0 - ye, dy);     // get_step(1-y, -dy)
-            xv[e] = acc[0][c] + acc[2][c];
+            xv[pe] = acc[0][c] + acc[2][c];
           }
           const double v2 = acc[1][c];
           if (ch == 0) x2a[c] = v2; else if (ch == 1) x2b[c] = v2; else if (ch == 2) x2c[c] = v2; else x2d[c] = v2;
@@ -830,6 +921,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
     double st = d1 > 0.0 ? n1 / d1 : 1e300, st2 = d2 > 0.0 ? n2 / d2 : 1e300;
     red.min2(g, st, st2);
     st = fmin(st > 1e299 ? 1.0 : st, st2 > 1e299 ? 1.0 : st2);
+    PC_PHASE(PC_PH_SWEEPB);
     // ---- sigma and the combined direction (every warp, redundantly: lanes own elements j, j + 32)
     const double z0 = v0 ? zc[j0] : 0.0, z1 = v1ok ? zc[j1] : 0.0;
     const double s0 = v0 ? scur[j0] : 0.0, s1 = v1ok ? scur[j1] : 0.0;
@@ -850,24 +942,27 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       ds1 = v1ok ? dsa1 - (s1 / z1) * (rc1 + dzc1) : 0.0;
       dtt = sc[1] + fma(sig, sc[2], sc[3]);
     }
+    PC_PHASE(PC_PH_SIGMA);
     // ---- dy = -D (ry + v1 + sigma v2 + v3), step bounds; du = v1 + sigma v2 + v3
     n1 = 1.0; d1 = 0.0; n2 = 1.0; d2 = 0.0;
 #pragma unroll 1
     for (int ch = 0; ch < NCH; ++ch) {
       const int cb = ch * 4 * T;
       if (cb >= n) break;
+      const int tc = pc_tc<T, IL>(cb, npad);
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         const int e = pc_col<T, VEC>(cb, g.tid, c);
+        const int pe = IL ? cb + c * tc + g.tid : e;
         const double v2 = (ch == 0) ? x2a[c] : (ch == 1) ? x2b[c] : (ch == 2) ? x2c[c] : x2d[c];
         if (e < n) {
-          const double ye = yv[e];
-          const double du = fma(sig, v2, xv[e]);
-          const double dy = -dweight(ye) * (rv[e] + du);
+          const double ye = yv[pe];
+          const double du = fma(sig, v2, xv[pe]);
+          const double dy = -dweight(ye) * (rv[pe] + du);
           if (dy < 0.0) ratio_min(n1, d1, ye, -dy);
           if (dy > 0.0) ratio_min(n2, d2, 1.0 - ye, dy);
-          if (V3) xv[e] = du;            // ry stays in rv; dy is recomputed in the update
-          else { xv[e] = dy; rv[e] = du; }
+          if (V3) xv[pe] = du;            // ry stays in rv; dy is recomputed in the update
+          else { xv[pe] = dy; rv[pe] = du; }
         }
       }
     }
@@ -884,38 +979,47 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       if (g.lane == 0) sc[0] += a * dtt;
     }
     zsel ^= 1;
+    PC_PHASE(PC_PH_DIR2);
     // ---- y += a dy ; u += a du ; ry = logit(y) + u
     pr = 0.0;
 #pragma unroll 1
     for (int ch = 0; ch < NCH; ++ch) {
       const int cb = ch * 4 * T;
       if (cb >= n) break;
+      const int tc = pc_tc<T, IL>(cb, npad);
       // one warp per sample: keep the log / division body rolled (ncu, C3: 36 % of the warp cycles were
       // instruction-fetch stalls with the 4x unrolled body; many small CTAs at different code positions per SM)
 #pragma unroll (WPS == 1 ? 1 : 4)
       for (int c = 0; c < 4; ++c) {
         const int e = pc_col<T, VEC>(cb, g.tid, c);
+        const int pe = IL ? cb + c * tc + g.tid : e;
         if (e < n) {
           if (V3) {
-            const double yo = yv[e], ro = rv[e], du = xv[e];
+            const double yo = yv[pe], ro = rv[pe], du = xv[pe];
             const double dy = -dweight(yo) * (ro + du);            // the expression of the pass above, same inputs
-            const double uo = ro - log(yo / (1.0 - yo));           // u = ry - logit(y)
             const double ye = fma(a, dy, yo);
-            const double ue = fma(a, du, uo);
-            const double r = log(ye / (1.0 - ye)) + ue;
-            yv[e] = ye; rv[e] = r;
+            double r;
+            if (A.twolog) {
+              const double uo = ro - log(yo / (1.0 - yo));         // u = ry - logit(y)
+              r = log(ye / (1.0 - ye)) + fma(a, du, uo);
+            } else {
+              // ry_new = logit(y_new) + u_old + a du = ry_old + a du + logit(y_new) - logit(y_old): one log, one division
+              r = fma(a, du, ro) + log((ye * (1.0 - yo)) / (yo * (1.0 - ye)));
+            }
+            yv[pe] = ye; rv[pe] = r;
             pr = fma(r, r, pr);
           } else {
-            const double ye = fma(a, xv[e], yv[e]);
-            const double ue = fma(a, rv[e], uv[e]);
+            const double ye = fma(a, xv[pe], yv[pe]);
+            const double ue = fma(a, rv[pe], uv[pe]);
             const double r = log(ye / (1.0 - ye)) + ue;
-            yv[e] = ye; uv[e] = ue; rv[e] = r;
+            yv[pe] = ye; uv[pe] = ue; rv[pe] = r;
             pr = fma(r, r, pr);
           }
         }
       }
     }
     pr = red.sum(g, pr);   // the barrier also publishes y / ry / z / s for the next sweep
+    PC_PHASE(PC_PH_UPDATE);
   }
   g.sync();
   const double* zfin = PCKV(1 + zsel);
@@ -923,7 +1027,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
   // ---- commit: y, lambda, prune (lam > thr), bookkeeping  (lib/bundle_entropy.py:228,234-237) -----------
   double bad = 0.0;
   for (int e = g.tid; e < n; e += T) {
-    const double ye = yv[e];
+    const double ye = yv[pc_pos<T, IL>(e, npad)];
     if (!isfinite(ye)) bad = 1.0;
     yu[e] = ye;
     b.y32[(size_t)u * n + e] = (float)ye;
@@ -959,6 +1063,7 @@ __global__ void __launch_bounds__(WPS * 32, WPS == 16 ? 1 : (R80 ? 24 : 16) / WP
       if (fin) stat_add(b.iter_stats, A.t, 5, 1.0);
     }
   }
+  PC_PHASE(PC_PH_COMMIT);
 #undef PCKV
 }
 

@@ -29,6 +29,7 @@ BUILDS = {
     "v3off": {"ICNN_PC_V3": "0"},  # 16-warp four-vector kernel, one sample per SM
     "legacy": {"ICNN_PC_LEGACY": "1"},
     "seed0": {"ICNN_PC_SEED": "0"},  # sweep A at it = 0 and the dependency residual pass always
+    "twolog": {"ICNN_PC_TWOLOG": "1"},  # V3 update with two logs per element
     # L2 prefetch distances of the V3 row sweeps, "sweep A trips,sweep B rows" (bundle_pc.cu)
     "pf0": {"ICNN_PC_PREFETCH": "0,0"},
     "pfa1": {"ICNN_PC_PREFETCH": "1,0"},
