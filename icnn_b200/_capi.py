@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 NSTAT = 8
 K2_PLAN_LEN = 8     # ICNN_K2_PLAN_LEN: int32 fields of an icnn_k2_plan / icnn_k2_last_launch record
 
@@ -36,6 +36,7 @@ SYMBOLS = [
     "icnn_train_grad_workspace_bytes", "icnn_train_grad",
     "icnn_conv_picnn_create", "icnn_conv_picnn_destroy", "icnn_conv_picnn_workspace_bytes", "icnn_conv_picnn_fg",
     "icnn_conv_solve_batch_fused", "icnn_conv_gd_solve",
+    "icnn_conv_train_grad_workspace_bytes", "icnn_conv_train_grad",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -79,6 +80,11 @@ class GdGrads(C.Structure):
 
 class TrainGrads(C.Structure):
     _fields_ = [("dWy", _fpp), ("dWz", _fpp), ("dcy", _fpp), ("dcz", _fpp), ("dd", _fpp)]
+
+
+class ConvTrainGrads(C.Structure):
+    _fields_ = [("dWz", _fpp), ("dWy", _fpp), ("dWred", _fpp), ("dbred", _fpp), ("dcy", _fpp), ("dcz", _fpp),
+                ("dd", _fpp)]
 
 
 class IcnnError(RuntimeError):
@@ -147,6 +153,10 @@ def _load():
     lib.icnn_conv_picnn_fg.argtypes = lib.icnn_picnn_fg.argtypes
     lib.icnn_conv_solve_batch_fused.argtypes = lib.icnn_solve_batch_fused.argtypes
     lib.icnn_conv_gd_solve.argtypes = lib.icnn_gd_solve.argtypes
+    lib.icnn_conv_train_grad_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int64]
+    lib.icnn_conv_train_grad_workspace_bytes.restype = C.c_size_t
+    lib.icnn_conv_train_grad.argtypes = [C.c_void_p, C.POINTER(Gates), C.POINTER(C.c_int64), C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.POINTER(ConvTrainGrads), C.c_void_p, C.c_void_p]
     for name in SYMBOLS:
         getattr(lib, name)  # AttributeError if the .so does not export it
     if lib.icnn_abi_version() != ABI_VERSION:

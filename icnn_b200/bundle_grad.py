@@ -19,6 +19,14 @@ training mode, the additive gates d_l enter through c E, so Wzx / bzx get a grad
 Parameter gradients are with respect to the handle's parameters, i.e. after an inference-mode batch-norm has been
 folded into the x-path weights (``PICNN.from_params``), as in ``gd_grad``.  Training-mode batch-norm is out of scope
 (DESIGN.md section 8).
+
+Both functions also take the convolutional PICNN of the image-completion experiment (``ConvPICNN.bind(x)``), whose
+training step is compute_gradients(F_, theta_) of completion/icnn_ebundle.py:129-140: the y-path gradients and
+gate adjoints come from ``icnn_conv_train_grad`` (icnn_b200/csrc/conv_train_grad.cu), the x-path ones from torch
+autograd through a grad-enabled recompute of ``ConvPICNN.gates`` on the bound minibatch (TF32 off).  The result is
+keyed by TensorFlow variable name with exactly the variables the reference's ``gv_`` holds, each in its own shape,
+so with ``return_device=True`` ``net.vars[k].grad = g`` works directly (then the optimiser step, ``proj``, and
+``net.update_weights()``).
 """
 from __future__ import annotations
 
@@ -30,6 +38,7 @@ import torch
 from . import _capi
 from .argmin_grad import LOSS, argmin_grad
 from .gd_grad import _f32, _xpath_backward
+from .conv_picnn import BoundConvPICNN, _no_tf32
 from .picnn import BoundPICNN
 
 # parameter names of the returned dictionary with x given (the PICNN attribute names)
@@ -37,10 +46,21 @@ PARAMS = ("Wy", "Wz", "Wu", "bu", "Wzu", "bzu", "Wyu", "byu", "Wzx", "bzx")
 
 
 def _check_fg(fg, who):
+    if isinstance(fg, BoundConvPICNN):
+        return
     if not isinstance(fg, BoundPICNN):
-        raise TypeError("%s needs a BoundPICNN (PICNN.bind(x))" % who)
+        raise TypeError("%s needs a BoundPICNN (PICNN.bind(x)) or a BoundConvPICNN (ConvPICNN.bind(x))" % who)
     if fg.affine:
         raise ValueError("%s: the affine RL wrapper has no bundle training step (RL/src/icnn.py:84)" % who)
+
+
+def _check_conv_x(fg, x, who):
+    """True for a conv fg (whose x-path uses the minibatch it was bound to: ``x`` is refused)."""
+    if not isinstance(fg, BoundConvPICNN):
+        return False
+    if x is not None:
+        raise ValueError("%s: a BoundConvPICNN uses the minibatch it was bound to; do not pass x" % who)
+    return True
 
 
 def _prepare(fg, offsets):
@@ -81,6 +101,76 @@ def _run(fg, Y, V, c, offsets, x, return_device):
     return {k: [host(t) for t in v] for k, v in grads.items()}
 
 
+def conv_trainable(net):
+    """Names of the TF variables the reference's gv_ holds for this conv net: every trainable variable except the
+    batch-norm statistics, the last u-layer (nothing consumes it) and the last conv layer's y_red (r_Lc is never
+    used), in the net's variable order."""
+    last_u = "u%d/" % (net.Lc + net.Ld - 1)
+    last_red = "z%d_y_red/" % (net.Lc - 1)
+    return [k for k in net.vars
+            if not k.endswith(("/moving_mean", "/moving_variance")) and not k.startswith((last_u, last_red))]
+
+
+def _conv_launch(fg, Y, V, c, offsets):
+    """icnn_conv_train_grad on the current stream (asynchronous): the output buffers, and what must outlive the work
+    under 'keep'."""
+    net, dev, B = fg.net, fg.net.device, fg.B
+    Lc, Ld, NL = net.Lc, net.Ld, net.Lc + net.Ld
+    R = int(offsets[-1])
+    Vr = net.vars
+    z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+    dWz = [None] + [z(*Vr["z%d_zu_proj/W" % i].shape) for i in range(1, NL)]
+    dWy = [z(*Vr["z%d_yu/W" % l].shape) for l in range(Lc)]
+    dWred = [z(*Vr["z%d_y_red/W" % l].shape) if l + 1 < Lc else None for l in range(Lc)]
+    dbred = [z(1) if l + 1 < Lc else None for l in range(Lc)]
+    dcy = [z(B, fg.cy[l][0].numel()) for l in range(Lc)]
+    dcz = [None] + [z(B, fg.cz[i][0].numel()) for i in range(1, NL)]
+    dd = [z(B, fg.d[i][0].numel()) for i in range(NL)]
+    arrs = [_capi.ptr_array(a) for a in (dWz, dWy, dWred, dbred, dcy, dcz, dd)]
+    gr = _capi.ConvTrainGrads(*[C.cast(a, _capi._fpp) for a in arrs])
+    off = (C.c_int64 * (B + 1))(*[int(o) for o in offsets])
+    ws = torch.empty(max(_capi.lib.icnn_conv_train_grad_workspace_bytes(net._h, B, R), 4), dtype=torch.uint8,
+                     device=dev)
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    _capi.check(_capi.lib.icnn_conv_train_grad(net._h, C.byref(fg.c_gates), off, Y.data_ptr(), V.data_ptr(),
+                                               c.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
+    return dict(dWz=dWz, dWy=dWy, dWred=dWred, dbred=dbred, dcy=dcy, dcz=dcz, dd=dd, keep=(arrs, gr, off, ws))
+
+
+def _conv_run(fg, Y, V, c, offsets, return_device):
+    net, B, Lc, NL = fg.net, fg.B, fg.net.Lc, fg.net.Lc + fg.net.Ld
+    o = _conv_launch(fg, Y, V, c, offsets)
+    dWz, dWy, dWred, dbred, dcy, dcz, dd = (o[k] for k in ("dWz", "dWy", "dWred", "dbred", "dcy", "dcz", "dd"))
+    Vr = net.vars
+    grads = {}
+    for i in range(1, NL):
+        grads["z%d_zu_proj/W" % i] = dWz[i]
+    for l in range(Lc):
+        grads["z%d_yu/W" % l] = dWy[l]
+        if l + 1 < Lc:
+            grads["z%d_y_red/W" % l] = dWred[l]
+            grads["z%d_y_red/b" % l] = dbred[l]
+    # x-path: d(sum of gate o gate adjoint)/d theta through the gates of the bound minibatch
+    names = [k for k in conv_trainable(net) if k not in grads]
+    P = {k: (v.detach().requires_grad_() if k in names else v) for k, v in Vr.items()}
+    # (cuDNN restricted to deterministic algorithms: two calls give the same bits)
+    with torch.enable_grad(), _no_tf32(), torch.backends.cudnn.flags(
+            enabled=torch.backends.cudnn.enabled, benchmark=False, deterministic=True, allow_tf32=False):
+        gz, gy, gd = net._gates(fg.x, P)
+        s = sum((gy[l].reshape(B, -1) * dcy[l]).sum() for l in range(Lc))
+        s = s + sum((gz[i].reshape(B, -1) * dcz[i]).sum() for i in range(1, NL))
+        s = s + sum((gd[i].reshape(B, -1) * dd[i]).sum() for i in range(NL))
+        xg = torch.autograd.grad(s, [P[k] for k in names])
+    grads.update(zip(names, (g.detach() for g in xg)))
+    grads = {k: grads[k] for k in conv_trainable(net)}
+    grads.update(dcy=dcy, dcz=dcz, dd=dd)
+    torch.cuda.current_stream().synchronize()      # ws / arrs / the inputs stay alive until the work is done
+    if return_device:
+        return grads
+    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
+    return {k: [host(t) for t in v] if isinstance(v, list) else host(v) for k, v in grads.items()}
+
+
 def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):
     """d (sum over the rows of F_) / d theta from the ``train_step_fd`` feeds.
 
@@ -91,8 +181,14 @@ def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):
     Returns the ``gd_grad`` dictionary layout: 'Wy', 'Wz' (per-layer lists, summed over all rows), the per-sample
     gate adjoints 'dcy', 'dcz', 'dd' ([B, .], summed over each sample's rows), and with ``x`` (the minibatch the
     gates were bound to) also 'Wu', 'bu', 'Wzu', 'bzu', 'Wyu', 'byu', 'Wzx', 'bzx'.  Gradients are with respect to
-    the handle's (batch-norm-folded) parameters."""
+    the handle's (batch-norm-folded) parameters.  Numpy arrays unless ``return_device``.
+
+    For a ``BoundConvPICNN``: {TF variable name: gradient in the variable's shape} over ``conv_trainable(net)``
+    (the x-path from the minibatch ``fg`` was bound to; ``x`` is refused), plus 'dcy' (per conv layer), 'dcz' and
+    'dd' (per layer, [B, flat gate]); numpy arrays, or with ``return_device=True`` torch tensors on the net's device
+    (for ``net.vars[k].grad = g``)."""
     _check_fg(fg, "train_grad")
+    conv = _check_conv_x(fg, x, "train_grad")
     net, dev, B = fg.net, fg.net.device, fg.B
     counts = np.asarray(counts.cpu() if isinstance(counts, torch.Tensor) else counts, dtype=np.int64).reshape(-1)
     if counts.shape != (B,) or (counts < 0).any():
@@ -103,6 +199,8 @@ def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):
         Yd, Vd, cd = _f32(Y, dev).reshape(-1, net.n), _f32(V, dev).reshape(-1, net.n), _f32(c, dev).reshape(-1)
         if Yd.shape[0] != R or Vd.shape[0] != R or cd.shape[0] != R:
             raise ValueError("train_grad: Y, V and c must have sum(counts) = %d rows" % R)
+        if conv:
+            return _conv_run(fg, Yd, Vd, cd, offsets, return_device)
         return _run(fg, Yd, Vd, cd, offsets, x, return_device)
 
 
@@ -113,6 +211,7 @@ def bundle_grad(fg: BoundPICNN, state, trueY, loss="xent", x=None, return_device
     ``keep_xs=True``, the default); ``trueY`` [B, n] the labels; ``loss`` 'xent' or 'mse'.  Same return layout as
     ``train_grad``."""
     _check_fg(fg, "bundle_grad")
+    conv = _check_conv_x(fg, x, "bundle_grad")
     if loss not in LOSS:
         raise ValueError("loss must be 'mse' or 'xent'")
     if state.B != fg.B or state.n != fg.net.n:
@@ -132,4 +231,6 @@ def bundle_grad(fg: BoundPICNN, state, trueY, loss="xent", x=None, return_device
         Y = state.ys[iu, slots].float()
         Vr = V[iu, ii].float()
         c = clam[iu, ii].float()
+        if conv:
+            return _conv_run(fg, Y.contiguous(), Vr.contiguous(), c.contiguous(), offsets, return_device)
         return _run(fg, Y.contiguous(), Vr.contiguous(), c.contiguous(), offsets, x, return_device)

@@ -215,8 +215,7 @@ class ConvPICNN:
         nbytes = _capi.lib.icnn_conv_picnn_workspace_bytes(self._h, int(B))
         return torch.empty(max(nbytes, 4), dtype=torch.uint8, device=self.device)
 
-    def _bn(self, u, i, channel_dim):
-        V = self.vars
+    def _bn(self, u, i, channel_dim, V):
         shape = [1] * u.dim()
         shape[channel_dim] = -1
         p = lambda nm: V["u%d/BatchNormalization/%s" % (i, nm)].reshape(shape)   # noqa: E731
@@ -226,34 +225,38 @@ class ConvPICNN:
         """x-path of Model.f (completion/icnn_ebundle.py:349-366,374-440) for x [B, H*W]: the gate lists of
         include/icnn_b200.h (conv maps NHWC), in float32 with TF32 off.  Batch-norm is applied as is, not folded:
         the next conv's zero padding sees the normalised values."""
-        V, Lc, Ld = self.vars, self.Lc, self.Ld
         x = torch.as_tensor(x, device=self.device).to(torch.float32)
+        with torch.no_grad(), _no_tf32():
+            return self._gates(x, self.vars)
+
+    def _gates(self, x, V):
+        """``gates`` on the weight dict ``V`` (differentiable in its tensors; the caller sets grad mode and TF32)."""
+        Lc, Ld = self.Lc, self.Ld
         B = int(x.shape[0])
         nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()                      # noqa: E731
         flat = lambda t: nhwc(t).reshape(B, -1) if t.dim() == 4 else t          # noqa: E731
         cy, cz, d = [None] * (Lc + Ld), [None] * (Lc + Ld), [None] * (Lc + Ld)
-        with torch.no_grad(), _no_tf32():
-            us, prev = [], x.reshape(B, 1, self.H, self.W)
-            for i, (_c, _k, s) in enumerate(self.convs):
-                prev = self._bn(torch.relu(_same_conv(prev, V["u%d/W" % i], V["u%d/b" % i], s)), i, 1)
-                us.append(prev)
-            for j, sz in enumerate(self.fcs):
-                i = Lc + j
-                prev = flat(prev) @ V["u%d/W" % i] + V["u%d/b" % i]
-                if sz != 1:
-                    prev = self._bn(torch.relu(prev), i, 1)
-                us.append(prev)
-            for i, (_c, _k, s) in enumerate(self.convs):
-                P = x.reshape(B, 1, self.H, self.W) if i == 0 else us[i - 1]
-                cy[i] = _same_conv(P, V["z%d_yu_u/W" % i], V["z%d_yu_u/b" % i], 1).reshape(B, -1).contiguous()
-                if i > 0:
-                    cz[i] = nhwc(torch.relu(_same_conv(P, V["z%d_zu_u/W" % i], V["z%d_zu_u/b" % i], 1)))
-                d[i] = nhwc(_same_conv(P, V["z%d_u/W" % i], V["z%d_u/b" % i], s))
-            for j in range(Ld):
-                i = Lc + j
-                P = flat(us[i - 1])
-                cz[i] = torch.relu(P @ V["z%d_zu_u/W" % i] + V["z%d_zu_u/b" % i]).contiguous()
-                d[i] = (P @ V["z%d_u/W" % i] + V["z%d_u/b" % i]).contiguous()
+        us, prev = [], x.reshape(B, 1, self.H, self.W)
+        for i, (_c, _k, s) in enumerate(self.convs):
+            prev = self._bn(torch.relu(_same_conv(prev, V["u%d/W" % i], V["u%d/b" % i], s)), i, 1, V)
+            us.append(prev)
+        for j, sz in enumerate(self.fcs):
+            i = Lc + j
+            prev = flat(prev) @ V["u%d/W" % i] + V["u%d/b" % i]
+            if sz != 1:
+                prev = self._bn(torch.relu(prev), i, 1, V)
+            us.append(prev)
+        for i, (_c, _k, s) in enumerate(self.convs):
+            P = x.reshape(B, 1, self.H, self.W) if i == 0 else us[i - 1]
+            cy[i] = _same_conv(P, V["z%d_yu_u/W" % i], V["z%d_yu_u/b" % i], 1).reshape(B, -1).contiguous()
+            if i > 0:
+                cz[i] = nhwc(torch.relu(_same_conv(P, V["z%d_zu_u/W" % i], V["z%d_zu_u/b" % i], 1)))
+            d[i] = nhwc(_same_conv(P, V["z%d_u/W" % i], V["z%d_u/b" % i], s))
+        for j in range(Ld):
+            i = Lc + j
+            P = flat(us[i - 1])
+            cz[i] = torch.relu(P @ V["z%d_zu_u/W" % i] + V["z%d_zu_u/b" % i]).contiguous()
+            d[i] = (P @ V["z%d_u/W" % i] + V["z%d_u/b" % i]).contiguous()
         return cz, cy, d
 
     def bind(self, x):
@@ -275,6 +278,7 @@ class BoundConvPICNN:
             self.c_gates = _capi.Gates(self.B, C.cast(self._cy, _capi._fpp), C.cast(self._cz, _capi._fpp),
                                        C.cast(self._d, _capi._fpp), 1.0, 0.0, 1.0)
             self.ws = net.workspace(self.B)
+            self.x = torch.as_tensor(x, device=net.device).to(torch.float32)   # the training gradient's x-path
 
     def fg_device(self, y32, f=None, g=None):
         """f [B], g [B, n] (float32 CUDA tensors) for a float32 CUDA iterate y32 [B, n]."""

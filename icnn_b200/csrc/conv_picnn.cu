@@ -17,34 +17,9 @@
 //             windows covering it in a fixed order (no atomics: bit-reproducible), fused with relu' o cz (delta_{l-1}
 //             as the next GEMM's hi/lo operand), cy o e_r and the transposed y_red convolution
 // The dense layers are K1's GEMMs with their epilogues; the width-1 output is a per-sample reduction.
-#include "tc_gemm.cuh"
+#include "conv_picnn.cuh"
 
 #include <cstring>
-
-namespace icnn {
-
-struct ConvGeom {
-  int C, k, s, Cp;            // out channels, kernel, stride, in channels of the z part (C_{l-1}; 0 at l = 0)
-  int Hi, Wi, Ho, Wo;         // input / output grid
-  int pt, pl;                 // 'SAME' padding before (top, left); the rest goes after
-  int K;                      // k^2 (Cp + 1)
-};
-
-}  // namespace icnn
-
-struct icnn_conv_picnn {
-  int H, W, Lc, Ld;
-  int fcs[ICNN_MAX_LAYERS];
-  icnn::ConvGeom g[ICNN_MAX_LAYERS];
-  int flat;                   // H_Lc * W_Lc * C_{Lc-1}: width of the first dense layer's input
-  // conv l: Wf [C, ld4(K)] (forward B operand), Wb [K, ld4(C)] (backward B operand); dense hidden layer j (index
-  // Lc + j): Wf [w, ld4(in)], Wb [in, ld4(w)]; all TF32 hi/lo
-  float* Wf_hi[2 * ICNN_MAX_LAYERS]; float* Wf_lo[2 * ICNN_MAX_LAYERS];
-  float* Wb_hi[2 * ICNN_MAX_LAYERS]; float* Wb_lo[2 * ICNN_MAX_LAYERS];
-  float* wout;                // [in] weights of the width-1 output layer
-  float* red[ICNN_MAX_LAYERS];  // [k^2 + 1]: Wred_l then bred_l
-  int in_w(int j) const { return j == 0 ? flat : fcs[j - 1]; }   // input width of dense layer j
-};
 
 namespace icnn {
 
@@ -168,10 +143,11 @@ __global__ void repitch_kernel(const float* shi, const float* slo, float* dhi, f
 //   e = sum over the output windows covering p (oy, then ox ascending) of cols[window, tap (Cp+1) + c]
 //   c < Cp:  delta_{l-1}[p, c] = relu'(z_{l-1}) cz_l e            -> TF32 hi/lo, row pitch ld4(Cp)
 //   c = Cp:  rho_l[p] = cy_l e + sum over the same windows of rho_{l+1} Wred_l[tap]   -> rho (l > 0) or the g row
+//   eout != nullptr (training gradient, conv_train_grad.cu): eout[p, c] = e, the un-gated adjoint [e_z | e_r]
 __global__ void col2im_kernel(const float* cols, ConvGeom g, int B, const float* Zp, const float* cz, float* dhi,
                               float* dlo, const float* cy, const float* rho_next, const float* wred, float* rho,
                               float* gout, long long g_row_stride, const int* perm, const int* count, int KS, int n,
-                              const int* skip) {
+                              float* eout, const int* skip) {
   if (skip != nullptr && *skip == 0) return;
   const int CC = g.Cp + 1;
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -194,6 +170,7 @@ __global__ void col2im_kernel(const float* cols, ConvGeom g, int B, const float*
       if (ych && rho_next) rr = fmaf(rho_next[mo], wred[ky * g.k + kx], rr);
     }
   }
+  if (eout) eout[i] = e;
   if (!ych) {
     const long long idx = p * g.Cp + c;
     const float v = Zp[idx] > 0.f ? cz[idx] * e : 0.f, h = tf32_rn(v);
@@ -212,19 +189,9 @@ __global__ void col2im_kernel(const float* cols, ConvGeom g, int B, const float*
   }
 }
 
-// ---- workspace --------------------------------------------------------------------------------------------------
-struct ConvWs {
-  float* Ah[ICNN_MAX_LAYERS]; float* Al[ICNN_MAX_LAYERS]; float* Z[ICNN_MAX_LAYERS];
-  float* dh[ICNN_MAX_LAYERS]; float* dl[ICNN_MAX_LAYERS];            // delta_l, the GEMM operand [M_l, ld4(C_l)]
-  float* r[ICNN_MAX_LAYERS]; float* rho[ICNN_MAX_LAYERS];            // l >= 1: [B, H_l W_l]
-  float* cols;                                                       // [M_l, K_l], the largest layer
-  float* fAh[ICNN_MAX_LAYERS]; float* fAl[ICNN_MAX_LAYERS]; float* fZ[ICNN_MAX_LAYERS];   // dense hidden layers
-  float* fdh[ICNN_MAX_LAYERS]; float* fdl[ICNN_MAX_LAYERS];
-  float* th; float* tl;                                              // delta_{Lc-1} at pitch C before repitching
-};
-
+// ---- workspace ----------------------------------------------------------------------------------------------------
 // floats of workspace for B rows; with base != nullptr also the buffer addresses
-static size_t conv_ws_floats(const icnn_conv_picnn* h, int B, float* base, ConvWs* w) {
+size_t conv_ws_floats(const icnn_conv_picnn* h, int B, float* base, ConvWs* w) {
   size_t off = 0;
   auto take = [&](size_t nfl) { const size_t o = off; off += (nfl + 63) & ~(size_t)63; return base ? base + o : nullptr; };
   size_t cmax = 0;
@@ -253,7 +220,7 @@ static inline unsigned nblk(long long n) { return (unsigned)((n + 255) / 256); }
 
 int conv_fg(const icnn_conv_picnn* h, const icnn_gates* gt, const float* y32, float* f, float* g,
             long long g_row_stride, const int* perm, const int* count, int KS, void* workspace, const int* skip,
-            cudaStream_t st) {
+            cudaStream_t st, float* const* eout) {
   const int B = gt->B, Lc = h->Lc, Ld = h->Ld, n = h->H * h->W;
   ConvWs w{};
   conv_ws_floats(h, B, static_cast<float*>(workspace), &w);
@@ -320,14 +287,24 @@ int conv_fg(const icnn_conv_picnn* h, const icnn_gates* gt, const float* y32, fl
     col2im_kernel<<<nblk((long long)B * G.Hi * G.Wi * (G.Cp + 1)), 256, 0, st>>>(
         w.cols, G, B, l ? w.Z[l - 1] : nullptr, gt->cz[l], l ? w.dh[l - 1] : nullptr, l ? w.dl[l - 1] : nullptr,
         gt->cy[l], l + 1 < Lc ? w.rho[l + 1] : nullptr, h->red[l], l ? w.rho[l] : nullptr, g, g_row_stride, perm,
-        count, KS, n, skip);
+        count, KS, n, eout ? eout[l] : nullptr, skip);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("conv_picnn_fg launch: %s", cudaGetErrorString(e)); return ICNN_E_CUDA; }
   return ICNN_OK;
 }
 
-static int check_gates(const icnn_conv_picnn* h, const icnn_gates* gt) {
+void conv_im2col_gate_launch(const float* Z, const float* cz, const float* r, const float* cy, const ConvGeom& g,
+                             int B, float* hi, float* lo, cudaStream_t st) {
+  im2col_gate_kernel<<<nblk((long long)B * g.Ho * g.Wo * g.K), 256, 0, st>>>(Z, cz, r, cy, g, B, hi, lo, nullptr);
+}
+
+void conv_gate_split_launch(const float* Z, const float* cz, int B, int w, float* hi, float* lo, int ld,
+                            cudaStream_t st) {
+  gate_split_kernel<<<nblk((long long)B * w), 256, 0, st>>>(Z, cz, B, w, hi, lo, ld, nullptr);
+}
+
+int conv_check_gates(const icnn_conv_picnn* h, const icnn_gates* gt) {
   ICNN_REQUIRE(gt->B > 0, "empty batch");
   ICNN_REQUIRE(gt->cy && gt->cz && gt->d, "null gate array");
   ICNN_REQUIRE(gt->in_scale == 1.f && gt->in_shift == 0.f && gt->g_scale == 1.f,
@@ -433,7 +410,7 @@ extern "C" int icnn_conv_picnn_fg(const icnn_conv_picnn_t* h, const icnn_gates* 
                                   int32_t KS, void* workspace, const int32_t* skip_if_zero, void* stream) {
   ICNN_REQUIRE(h && gates && y32 && f && g && workspace, "null pointer");
   ICNN_REQUIRE((perm == nullptr) == (count == nullptr), "perm and count go together");
-  int rc = check_gates(h, gates);
+  int rc = conv_check_gates(h, gates);
   if (rc) return rc;
   return conv_fg(h, gates, y32, f, g, g_row_stride, perm, count, KS, workspace, skip_if_zero,
                  static_cast<cudaStream_t>(stream));
@@ -447,7 +424,7 @@ extern "C" int icnn_conv_solve_batch_fused(const icnn_conv_picnn_t* h, const icn
   ICNN_REQUIRE(h->H * h->W == b->n, "H * W != bufs.n");
   ICNN_REQUIRE(cfg->nIter >= 1, "nIter < 1");
   ICNN_REQUIRE(b->KS >= 2, "KS < 2");
-  int rc = check_gates(h, gates);
+  int rc = conv_check_gates(h, gates);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if ((rc = icnn_bundle_init(b, cfg->nIter, stream))) return rc;
@@ -463,7 +440,7 @@ extern "C" int icnn_conv_gd_solve(const icnn_conv_picnn_t* h, const icnn_gates* 
                                   void* stream) {
   ICNN_REQUIRE(h && gates && y32 && v && g && f_out && workspace, "null pointer");
   ICNN_REQUIRE(nIter >= 0, "nIter < 0");
-  int rc = check_gates(h, gates);
+  int rc = conv_check_gates(h, gates);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int n = h->H * h->W;

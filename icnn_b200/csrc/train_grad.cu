@@ -24,55 +24,12 @@
 // weight-gradient GEMM's float64 variant, GdbW64) and rounded once at the end: the rows of a sample partly cancel
 // (its c sum to zero), so float32 sums would make the result depend on where the chunks are cut.
 #include "gdb.cuh"
-
-#include <cstdlib>
+#include "train_rows.cuh"
 
 namespace icnn {
 
 void picnn_gdb_tc_gate_a(const icnn_picnn* h, const icnn_gates* gt, const float* a, const GdbTcBufs& b, cudaStream_t st);
 size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* base);
-
-__global__ void round_to_float_kernel(float* dst, const double* src, long long N) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < N) dst[i] = (float)src[i];
-}
-
-// sample of each chunk row: the u in [u0, u1) with off[u] <= r0 + i < off[u + 1]
-__global__ void row_sample_kernel(int* row_u, const long long* off, int u0, int u1, long long r0, int rows) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= rows) return;
-  const long long r = r0 + i;
-  int lo = u0, hi = u1 - 1;   // largest u with off[u] <= r
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (off[mid] <= r) lo = mid; else hi = mid - 1;
-  }
-  row_u[i] = lo;
-}
-
-// dst[i, j] = src[row_u[i], j]
-__global__ void gather_rows_kernel(float* dst, const float* src, const int* row_u, long long N, int w) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < N) dst[i] = src[(long long)row_u[i / w] * w + i % w];
-}
-
-// out[u, j] += sum over the rows r of sample u inside [r0, r1) of scale[r] * src[r - r0, j]
-// (scale == nullptr: 1; src == nullptr: 1), rows in order.  Accumulated in float64: the bundle multipliers c of a
-// sample sum to zero (the KKT row of ones), so e.g. dd_L = sum_r c_r is pure cancellation and a float32 sum of
-// O(|c|) terms would leave rounding noise larger than the result.
-__global__ void segsum_kernel(float* out, const float* src, const float* scale, int w, const long long* off, int u0,
-                              int u1, long long r0, long long r1) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= (long long)(u1 - u0) * w) return;
-  const int u = u0 + (int)(i / w), j = (int)(i % w);
-  const long long a = off[u] > r0 ? off[u] : r0, b = off[u + 1] < r1 ? off[u + 1] : r1;
-  double acc = 0.0;
-  for (long long r = a; r < b; ++r) {
-    const double v = src ? (double)src[(r - r0) * w + j] : 1.0;
-    acc = scale ? fma((double)scale[r], v, acc) : acc + v;
-  }
-  out[(long long)u * w + j] = (float)((double)out[(long long)u * w + j] + acc);
-}
 
 struct TgLayout {
   size_t off, row_u;          // bytes: device copy of row_offsets, row -> sample map
@@ -99,17 +56,8 @@ static size_t tg_floats(const icnn_picnn* h, long long cap, TgLayout* t) {
 
 // rows per chunk: ICNN_TRAIN_CHUNK if set, else what fits ICNN_TRAIN_WS_GB (at least 64, at most R)
 static long long tg_chunk_rows(const icnn_picnn* h, long long R) {
-  if (const char* v = getenv("ICNN_TRAIN_CHUNK")) {
-    const long long c = atoll(v);
-    if (c > 0) return c < R ? c : R;
-  }
-  double gb = 2.0;
-  if (const char* v = getenv("ICNN_TRAIN_WS_GB")) gb = atof(v);
   const long long probe = 1024;
-  const double per_row = 4.0 * (double)(gdb_layout(h, (int)probe, 0).total + tg_floats(h, probe, nullptr)) / probe;
-  long long c = (long long)(gb * 1073741824.0 / per_row);
-  if (c < 64) c = 64;
-  return c < R ? c : R;
+  return chunk_rows(4.0 * (double)(gdb_layout(h, (int)probe, 0).total + tg_floats(h, probe, nullptr)) / probe, R);
 }
 
 static TgLayout tg_layout(const icnn_picnn* h, int B, long long R) {
@@ -214,15 +162,9 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
   long long r0 = 0;
   int u0 = 0;
   while (r0 < R) {
-    while (row_offsets[u0 + 1] <= r0) ++u0;     // first sample with rows left
-    // balanced chunks: k = ceil(rest / cap) pieces of about rest / k rows, cut at the first sample boundary
-    // past that size that still fits the cap; a single sample longer than the cap is split
-    const long long rest = R - r0, k = (rest + t.cap - 1) / t.cap, target = (rest + k - 1) / k;
-    long long r1 = r0;
-    int u1 = u0;
-    while (u1 < B && row_offsets[u1 + 1] - r0 <= t.cap && r1 - r0 < target) r1 = row_offsets[++u1];
-    if (r1 == r0) { r1 = r0 + t.cap; u1 = u0 + 1; }
-    else while (u1 < B && row_offsets[u1] < r1) ++u1;   // (u1 = one past the last sample with rows in the chunk)
+    long long r1;
+    int u1;
+    next_chunk(row_offsets, B, R, t.cap, r0, &u0, &r1, &u1);
     const int rows = (int)(r1 - r0);
 
     GdbLayout lo = t.lo;
@@ -257,11 +199,14 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
     const long long NS = (long long)(u1 - u0);
     for (int l = 0; l <= L; ++l) {
       const int wl = h->width(l), pl = h->prev(l);
-      segsum_kernel<<<(unsigned)((NS * n + 255) / 256), 256, 0, st>>>(gr->dcy[l], dcy[l], nullptr, n, off_d, u0, u1, r0, r1);
+      const SegView one{nullptr, nullptr, 0, 1, 0, 0};
+      segsum_prod_kernel<<<(unsigned)((NS * n + 255) / 256), 256, 0, st>>>(
+          gr->dcy[l], SegView{dcy[l], nullptr, n, n, 0, 0}, one, nullptr, n, off_d, u0, u1, r0, r1);
       if (l > 0)
-        segsum_kernel<<<(unsigned)((NS * pl + 255) / 256), 256, 0, st>>>(gr->dcz[l], dcz[l], nullptr, pl, off_d, u0, u1, r0, r1);
-      segsum_kernel<<<(unsigned)((NS * wl + 255) / 256), 256, 0, st>>>(gr->dd[l], l < L ? ws + lo.Dacc[l] : nullptr, c, wl,
-                                                                       off_d, u0, u1, r0, r1);
+        segsum_prod_kernel<<<(unsigned)((NS * pl + 255) / 256), 256, 0, st>>>(
+            gr->dcz[l], SegView{dcz[l], nullptr, pl, pl, 0, 0}, one, nullptr, pl, off_d, u0, u1, r0, r1);
+      segsum_prod_kernel<<<(unsigned)((NS * wl + 255) / 256), 256, 0, st>>>(
+          gr->dd[l], l < L ? SegView{ws + lo.Dacc[l], nullptr, wl, wl, 0, 0} : one, one, c, wl, off_d, u0, u1, r0, r1);
     }
     TG_LAUNCH("segmented sum");
     r0 = r1;

@@ -26,8 +26,9 @@
 extern "C" {
 #endif
 
-/* 7: icnn_bundle_bufs ends at iter_stats (the vec_ws scratch pointer of version 6 is gone; 19 pointers) */
-#define ICNN_ABI_VERSION 7
+/* 7: icnn_bundle_bufs ends at iter_stats (the vec_ws scratch pointer of version 6 is gone; 19 pointers)
+ * 8: the conv PICNN training gradient (icnn_conv_train_grads, icnn_conv_train_grad) */
+#define ICNN_ABI_VERSION 8
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -309,6 +310,31 @@ int icnn_conv_solve_batch_fused(const icnn_conv_picnn_t* h, const icnn_gates* ga
  * arguments are those of icnn_gd_solve. */
 int icnn_conv_gd_solve(const icnn_conv_picnn_t* h, const icnn_gates* gates, float* y32, float* v, float* g,
                        float* f_out, int32_t nIter, float lr, float momentum, void* workspace, void* stream);
+
+/* replaces: compute_gradients(F_, theta_) of the completion experiment (completion/icnn_ebundle.py:129-140) on
+ * F_ = c E(x, y) + sum_j v_j dE/dy_j, summed over the train_step_fd rows (:315-335), for this energy.  The rows
+ * and the gates follow icnn_train_grad: row_offsets (host, [B + 1], CSR), Y, V [R, H*W], c [R] device f32, gates
+ * the per-sample gates of the minibatch.  Outputs (host arrays of device f32 pointers, all overwritten):
+ *   dWz[Lc + Ld]   conv l: [k, k, C_{l-1}, C_l] (dWz[0] unused), dense: [in, out]       summed over every row
+ *   dWy[Lc]        [k, k, 1, C_l]
+ *   dWred[Lc]      [k, k, 1, 1], dbred[Lc] [1]; entry Lc-1 unused (r_{Lc} feeds nothing)
+ *   dcy[Lc], dcz[Lc + Ld] (dcz[0] unused), dd[Lc + Ld]   per sample, in the gate layouts above
+ * The x-path parameters follow from (dcy, dcz, dd) by backprop through the gates on the caller's side.
+ * workspace = icnn_conv_train_grad_workspace_bytes(h, B, R) device bytes; rows are processed in chunks bounded as
+ * for icnn_train_grad (ICNN_TRAIN_WS_GB, default 2 GiB; ICNN_TRAIN_CHUNK). */
+typedef struct {
+  float* const* dWz;
+  float* const* dWy;
+  float* const* dWred;
+  float* const* dbred;
+  float* const* dcy;
+  float* const* dcz;
+  float* const* dd;
+} icnn_conv_train_grads;
+size_t icnn_conv_train_grad_workspace_bytes(const icnn_conv_picnn_t* h, int32_t B, int64_t R);
+int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates* gates, const int64_t* row_offsets,
+                         const float* Y, const float* V, const float* c, const icnn_conv_train_grads* grads,
+                         void* workspace, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------ */
 /* Self test of the wgmma / TMA GEMM the tensor-core K1 path is built from:
