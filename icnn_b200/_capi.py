@@ -13,7 +13,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 NSTAT = 8
 K2_PLAN_LEN = 8     # ICNN_K2_PLAN_LEN: int32 fields of an icnn_k2_plan / icnn_k2_last_launch record
 
@@ -37,6 +37,7 @@ SYMBOLS = [
     "icnn_conv_picnn_create", "icnn_conv_picnn_destroy", "icnn_conv_picnn_workspace_bytes", "icnn_conv_picnn_fg",
     "icnn_conv_solve_batch_fused", "icnn_conv_gd_solve",
     "icnn_conv_train_grad_workspace_bytes", "icnn_conv_train_grad",
+    "icnn_conv_gd_backward_workspace_bytes", "icnn_conv_gd_backward",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -157,6 +158,11 @@ def _load():
     lib.icnn_conv_train_grad_workspace_bytes.restype = C.c_size_t
     lib.icnn_conv_train_grad.argtypes = [C.c_void_p, C.POINTER(Gates), C.POINTER(C.c_int64), C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.POINTER(ConvTrainGrads), C.c_void_p, C.c_void_p]
+    lib.icnn_conv_gd_backward_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.icnn_conv_gd_backward_workspace_bytes.restype = C.c_size_t
+    lib.icnn_conv_gd_backward.argtypes = [C.c_void_p, C.POINTER(Gates), C.c_void_p, C.c_void_p, C.c_float, C.c_int32,
+                                          C.c_float, C.c_float, C.c_void_p, C.POINTER(ConvTrainGrads), C.c_void_p,
+                                          C.c_void_p]
     for name in SYMBOLS:
         getattr(lib, name)  # AttributeError if the .so does not export it
     if lib.icnn_abi_version() != ABI_VERSION:

@@ -38,7 +38,7 @@ import torch
 from . import _capi
 from .argmin_grad import LOSS, argmin_grad
 from .gd_grad import _f32, _xpath_backward
-from .conv_picnn import BoundConvPICNN, _no_tf32
+from .conv_picnn import BoundConvPICNN, _gate_vjp, _to_host, _train_grad_buffers, _ypath_grads, conv_trainable
 from .picnn import BoundPICNN
 
 # parameter names of the returned dictionary with x given (the PICNN attribute names)
@@ -101,74 +101,32 @@ def _run(fg, Y, V, c, offsets, x, return_device):
     return {k: [host(t) for t in v] for k, v in grads.items()}
 
 
-def conv_trainable(net):
-    """Names of the TF variables the reference's gv_ holds for this conv net: every trainable variable except the
-    batch-norm statistics, the last u-layer (nothing consumes it) and the last conv layer's y_red (r_Lc is never
-    used), in the net's variable order."""
-    last_u = "u%d/" % (net.Lc + net.Ld - 1)
-    last_red = "z%d_y_red/" % (net.Lc - 1)
-    return [k for k in net.vars
-            if not k.endswith(("/moving_mean", "/moving_variance")) and not k.startswith((last_u, last_red))]
-
-
 def _conv_launch(fg, Y, V, c, offsets):
     """icnn_conv_train_grad on the current stream (asynchronous): the output buffers, and what must outlive the work
     under 'keep'."""
     net, dev, B = fg.net, fg.net.device, fg.B
-    Lc, Ld, NL = net.Lc, net.Ld, net.Lc + net.Ld
     R = int(offsets[-1])
-    Vr = net.vars
-    z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-    dWz = [None] + [z(*Vr["z%d_zu_proj/W" % i].shape) for i in range(1, NL)]
-    dWy = [z(*Vr["z%d_yu/W" % l].shape) for l in range(Lc)]
-    dWred = [z(*Vr["z%d_y_red/W" % l].shape) if l + 1 < Lc else None for l in range(Lc)]
-    dbred = [z(1) if l + 1 < Lc else None for l in range(Lc)]
-    dcy = [z(B, fg.cy[l][0].numel()) for l in range(Lc)]
-    dcz = [None] + [z(B, fg.cz[i][0].numel()) for i in range(1, NL)]
-    dd = [z(B, fg.d[i][0].numel()) for i in range(NL)]
-    arrs = [_capi.ptr_array(a) for a in (dWz, dWy, dWred, dbred, dcy, dcz, dd)]
-    gr = _capi.ConvTrainGrads(*[C.cast(a, _capi._fpp) for a in arrs])
-    off = (C.c_int64 * (B + 1))(*[int(o) for o in offsets])
+    o, gr, arrs = _train_grad_buffers(fg)
+    off = (C.c_int64 * (B + 1))(*[int(o_) for o_ in offsets])
     ws = torch.empty(max(_capi.lib.icnn_conv_train_grad_workspace_bytes(net._h, B, R), 4), dtype=torch.uint8,
                      device=dev)
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     _capi.check(_capi.lib.icnn_conv_train_grad(net._h, C.byref(fg.c_gates), off, Y.data_ptr(), V.data_ptr(),
                                                c.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
-    return dict(dWz=dWz, dWy=dWy, dWred=dWred, dbred=dbred, dcy=dcy, dcz=dcz, dd=dd, keep=(arrs, gr, off, ws))
+    return dict(o, keep=(arrs, gr, off, ws))
 
 
 def _conv_run(fg, Y, V, c, offsets, return_device):
-    net, B, Lc, NL = fg.net, fg.B, fg.net.Lc, fg.net.Lc + fg.net.Ld
+    net = fg.net
     o = _conv_launch(fg, Y, V, c, offsets)
-    dWz, dWy, dWred, dbred, dcy, dcz, dd = (o[k] for k in ("dWz", "dWy", "dWred", "dbred", "dcy", "dcz", "dd"))
-    Vr = net.vars
-    grads = {}
-    for i in range(1, NL):
-        grads["z%d_zu_proj/W" % i] = dWz[i]
-    for l in range(Lc):
-        grads["z%d_yu/W" % l] = dWy[l]
-        if l + 1 < Lc:
-            grads["z%d_y_red/W" % l] = dWred[l]
-            grads["z%d_y_red/b" % l] = dbred[l]
+    grads = _ypath_grads(net, o)
     # x-path: d(sum of gate o gate adjoint)/d theta through the gates of the bound minibatch
     names = [k for k in conv_trainable(net) if k not in grads]
-    P = {k: (v.detach().requires_grad_() if k in names else v) for k, v in Vr.items()}
-    # (cuDNN restricted to deterministic algorithms: two calls give the same bits)
-    with torch.enable_grad(), _no_tf32(), torch.backends.cudnn.flags(
-            enabled=torch.backends.cudnn.enabled, benchmark=False, deterministic=True, allow_tf32=False):
-        gz, gy, gd = net._gates(fg.x, P)
-        s = sum((gy[l].reshape(B, -1) * dcy[l]).sum() for l in range(Lc))
-        s = s + sum((gz[i].reshape(B, -1) * dcz[i]).sum() for i in range(1, NL))
-        s = s + sum((gd[i].reshape(B, -1) * dd[i]).sum() for i in range(NL))
-        xg = torch.autograd.grad(s, [P[k] for k in names])
-    grads.update(zip(names, (g.detach() for g in xg)))
+    grads.update(_gate_vjp(fg, names, o["dcy"], o["dcz"], o["dd"]))
     grads = {k: grads[k] for k in conv_trainable(net)}
-    grads.update(dcy=dcy, dcz=dcz, dd=dd)
+    grads.update(dcy=o["dcy"], dcz=o["dcz"], dd=o["dd"])
     torch.cuda.current_stream().synchronize()      # ws / arrs / the inputs stay alive until the work is done
-    if return_device:
-        return grads
-    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
-    return {k: [host(t) for t in v] if isinstance(v, list) else host(v) for k, v in grads.items()}
+    return grads if return_device else _to_host(grads)
 
 
 def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):

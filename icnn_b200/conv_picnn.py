@@ -301,3 +301,79 @@ class BoundConvPICNN:
         y32 = torch.as_tensor(np.ascontiguousarray(y, dtype=np.float32), device=self.net.device)
         f, g = self.fg_device(y32)
         return f.cpu().numpy(), g.cpu().numpy()
+
+
+# ---- shared by the training gradients (bundle_grad: the bundle-entropy mode, gd_grad: the back-optimisation mode) ----
+
+def conv_trainable(net):
+    """Names of the TF variables the reference's gv_ holds for this conv net: every trainable variable except the
+    batch-norm statistics, the last u-layer (nothing consumes it) and the last conv layer's y_red (r_Lc is never
+    used), in the net's variable order."""
+    last_u = "u%d/" % (net.Lc + net.Ld - 1)
+    last_red = "z%d_y_red/" % (net.Lc - 1)
+    return [k for k in net.vars
+            if not k.endswith(("/moving_mean", "/moving_variance")) and not k.startswith((last_u, last_red))]
+
+
+def conv_gd_trainable(net):
+    """Names of the TF variables the gv_ of the back-optimisation mode holds (completion/icnn.back.py:153-155, the
+    gradient of the loss through the unrolled GD steps, which see E only through dE/dy): ``conv_trainable`` without
+    the output layer's additive gate 'z{NL-1}_u/*', which dE/dy does not depend on.  The other layers' additive gates
+    'z{l}_u/*' pass through a ReLU, so TensorFlow connects them to the loss, with a gradient that is exactly zero."""
+    out_d = "z%d_u/" % (net.Lc + net.Ld - 1)
+    return [k for k in conv_trainable(net) if not k.startswith(out_d)]
+
+
+def _train_grad_buffers(fg):
+    """Output buffers of one icnn_conv_train_grad / icnn_conv_gd_backward call on ``fg``'s minibatch: a dict of the
+    per-layer lists 'dWz', 'dWy', 'dWred', 'dbred' (in the variables' shapes), 'dcy', 'dcz', 'dd' ([B, flat gate]),
+    and the ConvTrainGrads struct with the pointer arrays it points into (these must outlive the work)."""
+    net, dev, B = fg.net, fg.net.device, fg.B
+    Lc, NL = net.Lc, net.Lc + net.Ld
+    Vr = net.vars
+    z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+    o = dict(dWz=[None] + [z(*Vr["z%d_zu_proj/W" % i].shape) for i in range(1, NL)],
+             dWy=[z(*Vr["z%d_yu/W" % l].shape) for l in range(Lc)],
+             dWred=[z(*Vr["z%d_y_red/W" % l].shape) if l + 1 < Lc else None for l in range(Lc)],
+             dbred=[z(1) if l + 1 < Lc else None for l in range(Lc)],
+             dcy=[z(B, fg.cy[l][0].numel()) for l in range(Lc)],
+             dcz=[None] + [z(B, fg.cz[i][0].numel()) for i in range(1, NL)],
+             dd=[z(B, fg.d[i][0].numel()) for i in range(NL)])
+    arrs = [_capi.ptr_array(o[k]) for k in ("dWz", "dWy", "dWred", "dbred", "dcy", "dcz", "dd")]
+    gr = _capi.ConvTrainGrads(*[C.cast(a, _capi._fpp) for a in arrs])
+    return o, gr, arrs
+
+
+def _ypath_grads(net, o):
+    """{TF variable name: gradient} of the y-path weights from the buffers of ``_train_grad_buffers``."""
+    Lc, NL = net.Lc, net.Lc + net.Ld
+    grads = {}
+    for i in range(1, NL):
+        grads["z%d_zu_proj/W" % i] = o["dWz"][i]
+    for l in range(Lc):
+        grads["z%d_yu/W" % l] = o["dWy"][l]
+        if l + 1 < Lc:
+            grads["z%d_y_red/W" % l] = o["dWred"][l]
+            grads["z%d_y_red/b" % l] = o["dbred"][l]
+    return grads
+
+
+def _gate_vjp(fg, names, dcy, dcz, dd):
+    """{k: d(sum over the gates of gate o adjoint) / d net.vars[k]} for k in ``names``: the x-path gradients, by torch
+    autograd through a grad-enabled recompute of ``ConvPICNN._gates`` on the minibatch ``fg`` was bound to, with TF32
+    off and cuDNN restricted to deterministic algorithms (two calls give the same bits)."""
+    net, B, Lc, NL = fg.net, fg.B, fg.net.Lc, fg.net.Lc + fg.net.Ld
+    P = {k: (v.detach().requires_grad_() if k in names else v) for k, v in net.vars.items()}
+    with torch.enable_grad(), _no_tf32(), torch.backends.cudnn.flags(
+            enabled=torch.backends.cudnn.enabled, benchmark=False, deterministic=True, allow_tf32=False):
+        gz, gy, gd = net._gates(fg.x, P)
+        s = sum((gy[l].reshape(B, -1) * dcy[l]).sum() for l in range(Lc))
+        s = s + sum((gz[i].reshape(B, -1) * dcz[i]).sum() for i in range(1, NL))
+        s = s + sum((gd[i].reshape(B, -1) * dd[i]).sum() for i in range(NL))
+        xg = torch.autograd.grad(s, [P[k] for k in names])
+    return dict(zip(names, (g.detach() for g in xg)))
+
+
+def _to_host(grads):
+    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
+    return {k: [host(t) for t in v] if isinstance(v, list) else host(v) for k, v in grads.items()}

@@ -30,9 +30,17 @@
 // A conv layer's reduction is long (rows H_{l+1} W_{l+1}) and its output small (K_l x C_l), so the reduction is
 // split over the rows into enough CTAs to fill the machine (wsplit_kernel), and the float64 partials are summed in
 // a fixed order (ws_reduce_kernel): no atomics, the same result on every call.
+//
+// The GD training backward of the same net (icnn_conv_gd_backward, completion/icnn.back.py:133-156) is this gradient
+// on other rows: with a = dloss/dy_N and kappa_i of gd_backward.cu's derivation (the conv energy is piecewise linear
+// in y too), dloss/dtheta = sum_{i < N} d/dtheta <dE/dy(x, y_i), kappa_i a>, i.e. one row per (sample, GD step) with
+// Y = y_i, V = kappa_i a, c = 0.  It runs the GD loop of icnn_conv_gd_solve keeping the iterates, forms the rows
+// and calls icnn_conv_train_grad on them; with c = 0 the hats are the tangents and dd, dbred come back zero.
 #include "conv_picnn.cuh"
 #include "gdb.cuh"
 #include "train_rows.cuh"
+
+#include <vector>
 
 namespace icnn {
 
@@ -317,6 +325,58 @@ static int wgrad_split(WsArgs a, double* acc, cudaStream_t st) {
   return ICNN_OK;
 }
 
+// every per-layer buffer of icnn_conv_train_grads the layers use is given
+static int ctg_check_buffers(const icnn_conv_picnn* h, const icnn_conv_train_grads* gr) {
+  const int Lc = h->Lc, NL = h->Lc + h->Ld;
+  for (int i = 0; i < NL; ++i) {
+    ICNN_REQUIRE(gr->dd[i] && (i == 0 || (gr->dWz[i] && gr->dcz[i])), "null gradient buffer");
+    ICNN_REQUIRE(i >= Lc || (gr->dWy[i] && gr->dcy[i]), "null gradient buffer");
+    ICNN_REQUIRE(i + 1 >= Lc || (gr->dWred[i] && gr->dbred[i]), "null gradient buffer");
+  }
+  return ICNN_OK;
+}
+
+// ---- the GD training backward (icnn_conv_gd_backward) -------------------------------------------------------------
+// Its rows are one per (sample u, GD step i), sample-major: row u nIter + i holds Y = y_i[u], V = kappa_i a[u], c = 0,
+// so the row offsets are u nIter and the gradient is icnn_conv_train_grad on them.
+
+// V[u, i, :] = kappa_i a[u, :] with a = loss_scale (yN - trueY): one subtraction and one multiply for a, one
+// multiply for V; c [B nIter] = 0
+static __global__ void gd_seed_kernel(float* V, float* c, const float* yN, const float* trueY, const float* kappa,
+                                      float loss_scale, int nIter, int n, long long N) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const long long row = i / n, u = row / nIter;
+  const int j = (int)(i % n), it = (int)(row % nIter);
+  const float a = loss_scale * (yN[u * n + j] - trueY[u * n + j]);
+  V[i] = kappa[it] * a;
+  if (j == 0) c[row] = 0.f;
+}
+
+// bytes: the trajectory Y [B nIter, n], V [B nIter, n], c [B nIter], kappa [nIter], the GD loop's v, g [B, n] and
+// f [B]; then one region that the loop's conv_fg workspace and, after the loop, icnn_conv_train_grad's share
+struct CgdLayout { size_t Y, V, c, kap, v, g, f, ws, total; };
+
+static CgdLayout cgd_layout(const icnn_conv_picnn* h, int B, int nIter) {
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t R = (size_t)B * nIter, n = (size_t)h->H * h->W;
+  CgdLayout t{};
+  size_t bytes = 0;
+  auto take = [&](size_t nb_) { const size_t o = bytes; bytes += al(nb_ > 0 ? nb_ : 4); return o; };
+  t.Y = take(sizeof(float) * R * n);
+  t.V = take(sizeof(float) * R * n);
+  t.c = take(sizeof(float) * R);
+  t.kap = take(sizeof(float) * (size_t)nIter);
+  t.v = take(sizeof(float) * B * n);
+  t.g = take(sizeof(float) * B * n);
+  t.f = take(sizeof(float) * B);
+  ConvWs w{};
+  const size_t fgb = sizeof(float) * conv_ws_floats(h, B, nullptr, &w), tgb = ctg_layout(h, B, (long long)R).total;
+  t.ws = take(fgb > tgb ? fgb : tgb);
+  t.total = bytes;
+  return t;
+}
+
 }  // namespace icnn
 
 using namespace icnn;
@@ -339,11 +399,7 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
   const long long R = row_offsets[B];
   ICNN_REQUIRE(R <= INT32_MAX, "more than 2^31 - 1 rows");
   ICNN_REQUIRE(R == 0 || (Y && V && c), "null row input");
-  for (int i = 0; i < NL; ++i) {
-    ICNN_REQUIRE(gr->dd[i] && (i == 0 || (gr->dWz[i] && gr->dcz[i])), "null gradient buffer");
-    ICNN_REQUIRE(i >= Lc || (gr->dWy[i] && gr->dcy[i]), "null gradient buffer");
-    ICNN_REQUIRE(i + 1 >= Lc || (gr->dWred[i] && gr->dbred[i]), "null gradient buffer");
-  }
+  if ((rc = ctg_check_buffers(h, gr))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   // outputs: the per-sample ones accumulate over the chunks from zero
@@ -524,4 +580,59 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
   }
   CTG_LAUNCH("round");
   return ICNN_OK;
+}
+
+extern "C" size_t icnn_conv_gd_backward_workspace_bytes(const icnn_conv_picnn_t* h, int32_t B, int32_t nIter) {
+  if (!h || B <= 0 || nIter < 0 || (long long)B * nIter > INT32_MAX) return 0;
+  return cgd_layout(h, B, nIter).total;
+}
+
+extern "C" int icnn_conv_gd_backward(const icnn_conv_picnn_t* h, const icnn_gates* gates, const float* y0,
+                                     const float* trueY, float loss_scale, int32_t nIter, float lr, float momentum,
+                                     float* yN, const icnn_conv_train_grads* gr, void* workspace, void* stream) {
+  ICNN_REQUIRE(h && gates && y0 && trueY && yN && gr && workspace, "null pointer");
+  ICNN_REQUIRE(gr->dWz && gr->dWy && gr->dWred && gr->dbred && gr->dcy && gr->dcz && gr->dd, "null gradient array");
+  ICNN_REQUIRE(nIter >= 0, "nIter < 0");
+  int rc = conv_check_gates(h, gates);
+  if (rc) return rc;
+  const int B = gates->B, n = h->H * h->W;
+  ICNN_REQUIRE((long long)B * nIter <= INT32_MAX, "B * nIter is more than 2^31 - 1 rows");
+  if ((rc = ctg_check_buffers(h, gr))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const CgdLayout t = cgd_layout(h, B, nIter);
+  char* wsb = static_cast<char*>(workspace);
+  float* Y = reinterpret_cast<float*>(wsb + t.Y);
+  float* V = reinterpret_cast<float*>(wsb + t.V);
+  float* c = reinterpret_cast<float*>(wsb + t.c);
+  float* kap = reinterpret_cast<float*>(wsb + t.kap);
+  float* v = reinterpret_cast<float*>(wsb + t.v);
+  float* g = reinterpret_cast<float*>(wsb + t.g);
+  float* f = reinterpret_cast<float*>(wsb + t.f);
+  void* ws = wsb + t.ws;
+  const long long N = (long long)B * n, RN = N * nIter;
+
+  // ---- the GD loop of icnn_conv_gd_solve in yN, recording y_i at row u nIter + i before step i ----
+  ICNN_CUDA_CHECK(cudaMemcpyAsync(yN, y0, sizeof(float) * N, cudaMemcpyDeviceToDevice, st));
+  ICNN_CUDA_CHECK(cudaMemsetAsync(v, 0, sizeof(float) * N, st));
+  for (int it = 0; it < nIter; ++it) {
+    ICNN_CUDA_CHECK(cudaMemcpy2DAsync(Y + (size_t)it * n, sizeof(float) * (size_t)nIter * n, yN, sizeof(float) * n,
+                                      sizeof(float) * n, B, cudaMemcpyDeviceToDevice, st));
+    if ((rc = conv_fg(h, gates, yN, f, g, n, nullptr, nullptr, 0, ws, nullptr, st))) return rc;
+    gd_update_launch(yN, v, g, N, lr, momentum, st);
+  }
+
+  // ---- row seeds V = kappa_i a, c = 0 ----
+  std::vector<float> kappa(nIter > 0 ? nIter : 1, 0.f);
+  gd_kappa(nIter, lr, momentum, kappa.data());
+  if (nIter > 0) {
+    // (pageable source: the call returns once kappa has been staged)
+    ICNN_CUDA_CHECK(cudaMemcpyAsync(kap, kappa.data(), sizeof(float) * nIter, cudaMemcpyHostToDevice, st));
+    gd_seed_kernel<<<nb(RN), 256, 0, st>>>(V, c, yN, trueY, kap, loss_scale, nIter, n, RN);
+    CTG_LAUNCH("GD row seeds");
+  }
+
+  // ---- the training gradient of those rows: sample u owns rows [u nIter, (u + 1) nIter) ----
+  std::vector<int64_t> off((size_t)B + 1);
+  for (int u = 0; u <= B; ++u) off[u] = (int64_t)u * nIter;
+  return icnn_conv_train_grad(h, gates, off.data(), Y, V, c, gr, ws, stream);
 }

@@ -466,14 +466,8 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
   const unsigned gN = (unsigned)((N + 255) / 256);
 
   // adjoint weights of the nIter gradient evaluations
-  std::vector<double> c(nIter + 2, 0.0);
   std::vector<float> kappa(nIter > 0 ? nIter : 1, 0.f);
-  double ksum = 0.0;
-  if (nIter > 0) {
-    c[nIter] = 1.0 + (double)momentum;
-    for (int i = nIter - 1; i >= 1; --i) c[i] = (double)momentum * c[i + 1] + 1.0;
-    for (int i = 0; i < nIter; ++i) { kappa[i] = (float)(-(double)lr * c[i + 1]); ksum += (double)kappa[i]; }
-  }
+  const double ksum = gd_kappa(nIter, lr, momentum, kappa.data());
 
   // outputs and accumulators start from zero
   for (int l = 0; l <= L; ++l) {

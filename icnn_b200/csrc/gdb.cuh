@@ -37,4 +37,18 @@ int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const 
 // dst[r, j] += c[r] * src[r, j] for r < rows, j < w
 void launch_row_axpy(float* dst, const float* src, const float* c, long long rows, int w, cudaStream_t st);
 
+// Adjoint weights of the nIter gradient evaluations of the unrolled momentum-GD loop (gd_backward.cu's header), on
+// the host in double:  c_N = 1 + m,  c_i = m c_{i+1} + 1,  kappa[i] = float(-lr c_{i+1})  for i < nIter.
+// Returns the double sum of the float kappa[i], i = 0..nIter-1 in that order (0 for nIter = 0).
+inline double gd_kappa(int nIter, float lr, float momentum, float* kappa) {
+  double c = 1.0 + (double)momentum;   // c_{i+1} of i = nIter - 1
+  for (int i = nIter - 1; i >= 0; --i) {
+    kappa[i] = (float)(-(double)lr * c);
+    c = (double)momentum * c + 1.0;
+  }
+  double ksum = 0.0;
+  for (int i = 0; i < nIter; ++i) ksum += (double)kappa[i];
+  return ksum;
+}
+
 }  // namespace icnn

@@ -9,6 +9,12 @@ x-path parameters (Wu/bu, Wzu/bzu, Wyu/byu) follow from the gate adjoints by ord
 backprop, a handful of library GEMMs outside the hot loop.  The additive gate d_l does not enter
 dE/dy, so Wzx/bzx get no gradient (TF returns None for them, filtered at icnn-back.py:137-138).
 
+``gd_grad`` also takes the convolutional PICNN of the image-completion experiment (``ConvPICNN.bind(x)``), whose
+back-optimisation mode (completion/icnn.back.py:121-156) unrolls the same loop on the conv energy.  The y-path
+gradients and the gate adjoints come from ``icnn_conv_gd_backward`` (icnn_b200/csrc/conv_train_grad.cu: the loop, then
+the conv training gradient on one row per (sample, step)), the x-path ones from torch autograd through a
+grad-enabled recompute of the gates of the bound minibatch (TF32 off), as for ``bundle_grad``.
+
 ``makeCvx`` / ``proj`` (icnn-back.py:141-144) -- the projection of the 'proj' weights Wz onto the
 non-negative orthant applied after every optimiser step -- are ``make_cvx`` / ``proj`` below.
 """
@@ -20,6 +26,8 @@ import numpy as np
 import torch
 
 from . import _capi
+from .conv_picnn import (BoundConvPICNN, _gate_vjp, _to_host, _train_grad_buffers, _ypath_grads, conv_gd_trainable,
+                         conv_trainable)
 from .picnn import BoundPICNN
 
 
@@ -35,9 +43,21 @@ def gd_grad(fg: BoundPICNN, y0, trueY, nIter=30, lr=0.01, momentum=0.3, loss_sca
     and with ``x`` given also 'Wu', 'bu', 'Wzu', 'bzu', 'Wyu', 'byu') to per-layer lists, plus the
     gate adjoints 'dcy', 'dcz'.  ``loss_scale`` defaults to 2/(B n), i.e. the multi-label script's
     ``reduce_mean(square(yn - trueY))``; completion/icnn.back.py:150 is ``2 * 255**2 / (B n)``.
-    ``x`` [B, m] is the minibatch the gates were bound to (needed only for the x-path gradients)."""
+    ``x`` [B, m] is the minibatch the gates were bound to (needed only for the x-path gradients).
+
+    For a ``BoundConvPICNN`` (completion/icnn.back.py:121-156; its values are lr = 0.01, momentum = 0.9 (:133-134),
+    nIter = 30 (--nGdIter) and loss_scale = 2 * 255**2 / (B n) for ``reduce_mean(square(255 (yn - trueY)))``):
+    ``grads`` maps the TF variable names of ``conv_gd_trainable(net)`` -- exactly the reference's gv_ -- to gradients
+    in the variables' shapes, with the x-path from the minibatch ``fg`` was bound to (``x`` is refused), plus the gate
+    adjoints 'dcy' (per conv layer) and 'dcz' (per layer, [B, flat gate]).  The additive gates 'z{l}_u/*' and the
+    y_red biases 'z{l}_y_red/b' are in gv_ with a gradient that is exactly zero, and are returned as zeros.  Numpy
+    arrays, or with ``return_device=True`` torch tensors on the net's device (for ``net.vars[k].grad = g``)."""
+    if isinstance(fg, BoundConvPICNN):
+        if x is not None:
+            raise ValueError("gd_grad: a BoundConvPICNN uses the minibatch it was bound to; do not pass x")
+        return _conv_gd_grad(fg, y0, trueY, nIter, lr, momentum, loss_scale, return_device)
     if not isinstance(fg, BoundPICNN):
-        raise TypeError("gd_grad needs a BoundPICNN (PICNN.bind(x))")
+        raise TypeError("gd_grad needs a BoundPICNN (PICNN.bind(x)) or a BoundConvPICNN (ConvPICNN.bind(x))")
     if fg.affine:
         raise ValueError("gd_grad: the affine RL wrapper is not part of the icnn.back training graph")
     net, dev, B = fg.net, fg.net.device, fg.B
@@ -71,6 +91,37 @@ def gd_grad(fg: BoundPICNN, y0, trueY, nIter=30, lr=0.01, momentum=0.3, loss_sca
         return yN, grads
     host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
     return host(yN), {k: [host(t) for t in v] for k, v in grads.items()}
+
+
+def _conv_gd_grad(fg, y0, trueY, nIter, lr, momentum, loss_scale, return_device):
+    net, dev, B, n = fg.net, fg.net.device, fg.B, fg.net.n
+    with torch.cuda.device(dev):
+        y0d, tY = _f32(y0, dev), _f32(trueY, dev)
+        if tuple(y0d.shape) != (B, n) or tuple(tY.shape) != (B, n):
+            raise ValueError("gd_grad: y0 and trueY must be [%d, %d], got %s and %s"
+                             % (B, n, tuple(y0d.shape), tuple(tY.shape)))
+        if loss_scale is None:
+            loss_scale = 2.0 / (B * n)
+        o, gr, arrs = _train_grad_buffers(fg)
+        yN = torch.empty(B, n, dtype=torch.float32, device=dev)
+        ws = torch.empty(max(_capi.lib.icnn_conv_gd_backward_workspace_bytes(net._h, B, int(nIter)), 4),
+                         dtype=torch.uint8, device=dev)
+        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        _capi.check(_capi.lib.icnn_conv_gd_backward(net._h, C.byref(fg.c_gates), y0d.data_ptr(), tY.data_ptr(),
+                                                    float(loss_scale), int(nIter), float(lr), float(momentum),
+                                                    yN.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
+        grads = _ypath_grads(net, o)
+        # x-path through the gates of the bound minibatch, over the same variables as the bundle-entropy mode (so
+        # that the two give the same bits on the same rows); dd is zero, and the output layer's additive gate,
+        # which only dd reaches, is then dropped
+        names = [k for k in conv_trainable(net) if k not in grads]
+        grads.update(_gate_vjp(fg, names, o["dcy"], o["dcz"], o["dd"]))
+        grads = {k: grads[k] for k in conv_gd_trainable(net)}
+        grads.update(dcy=o["dcy"], dcz=o["dcz"])
+        torch.cuda.current_stream().synchronize()      # ws / arrs stay alive until the work is done
+    if return_device:
+        return yN, grads
+    return yN.cpu().numpy(), _to_host(grads)
 
 
 def _xpath_backward(net, x, dcy, dcz, dd=None):

@@ -27,8 +27,9 @@ extern "C" {
 #endif
 
 /* 7: icnn_bundle_bufs ends at iter_stats (the vec_ws scratch pointer of version 6 is gone; 19 pointers)
- * 8: the conv PICNN training gradient (icnn_conv_train_grads, icnn_conv_train_grad) */
-#define ICNN_ABI_VERSION 8
+ * 8: the conv PICNN training gradient (icnn_conv_train_grads, icnn_conv_train_grad)
+ * 9: the conv PICNN GD training backward (icnn_conv_gd_backward) */
+#define ICNN_ABI_VERSION 9
 
 #define ICNN_OK 0
 #define ICNN_E_INVALID (-1)  /* bad argument */
@@ -335,6 +336,22 @@ size_t icnn_conv_train_grad_workspace_bytes(const icnn_conv_picnn_t* h, int32_t 
 int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates* gates, const int64_t* row_offsets,
                          const float* Y, const float* V, const float* c, const icnn_conv_train_grads* grads,
                          void* workspace, void* stream);
+/* replaces: TensorFlow's double backprop behind opt.compute_gradients(self.mse_, self.theta_) of the completion
+ * experiment's back-optimisation mode (completion/icnn.back.py:133-156) for this energy: the nIter unrolled
+ * momentum-GD steps of icnn_conv_gd_solve (lr = 0.01, momentum = 0.9 at :133-134) from y0 [B, H*W], then
+ * mse_ = reduce_mean(square(255 (yn_ - trueY))) (:149).  The arguments are those of icnn_gd_backward: y_N goes to yN
+ * [B, H*W] (bit-identical to icnn_conv_gd_solve with the same arguments), a = loss_scale (y_N - trueY) is d loss /
+ * d y_N (completion: loss_scale = 2 255^2 / (B H W)).  Outputs in the icnn_conv_train_grads layouts, all overwritten:
+ * d loss / d (y-path weights) summed over the batch, and the per-sample gate adjoints dcy, dcz; dd and dbred come
+ * back zero (the additive gates do not enter dE/dy, and TensorFlow's graph gives the y_red bias a zero gradient).
+ * The gradient is that of icnn_conv_train_grad on one row per (sample, step): the rows are chunked the same way.
+ * workspace = icnn_conv_gd_backward_workspace_bytes(h, B, nIter) device bytes: the trajectory and the row seeds
+ * (2 B nIter H W floats) plus the chunked gradient's workspace; 0 for arguments it cannot size (B * nIter must be
+ * at most 2^31 - 1 rows).  nIter = 0 gives yN = y0 and zero gradients. */
+size_t icnn_conv_gd_backward_workspace_bytes(const icnn_conv_picnn_t* h, int32_t B, int32_t nIter);
+int icnn_conv_gd_backward(const icnn_conv_picnn_t* h, const icnn_gates* gates, const float* y0, const float* trueY,
+                          float loss_scale, int32_t nIter, float lr, float momentum, float* yN,
+                          const icnn_conv_train_grads* grads, void* workspace, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------ */
 /* Self test of the wgmma / TMA GEMM the tensor-core K1 path is built from:
