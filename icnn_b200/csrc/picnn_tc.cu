@@ -171,6 +171,109 @@ struct TcSmem {
   static_assert(TC_BM * (BN + 1) * 4 <= BAR_OFF, "epilogue tile does not fit the ring");
 };
 
+// ---- fused epilogue of one output element (m, nn), shared by the single-tile and split-K paths ----
+// Global inputs of the element, loaded by tc_epi_load before any arithmetic so that the single-tile path can issue the
+// loads of a whole row group first:
+//   mode 0: v0 = D (bias; the primal activation for tangent 1), v1 = Cz_next; GDB tangent 2: v2 = Zmask
+//   mode 1, column < N0: v0 = Zprev, v1 = Cz; GDB: v2 = Ztprev, v3 = dCz, v4 = Dacc (old values)
+//   mode 1, g column: v0 = Cy, v1 = g (old value)
+//   mode 3: v0 = bias
+template <bool GDB> struct TcEpiIn { float v0 = 0.f, v1 = 0.f; };
+template <> struct TcEpiIn<true> : TcEpiIn<false> { float v2, v3, v4; };
+
+// mode 1: row m of g, at the plain row stride or, with perm, in the bundle slot perm[m, count[m]]
+__device__ __forceinline__ float* tc_g_row(const TcArgs& a, int m) {
+  return (a.perm == nullptr) ? a.g + (long long)m * a.g_row_stride
+                             : a.g + ((long long)m * a.KS + a.perm[(long long)m * a.KS + a.count[m]]) * a.n;
+}
+
+template <bool GDB>
+__device__ __forceinline__ TcEpiIn<GDB> tc_epi_load(const TcArgs& a, int m, int nn, const float* grow) {
+  TcEpiIn<GDB> in;
+  if (a.mode == 0) {
+    const long long idx = (long long)m * a.N + nn;
+    long long didx = idx;
+    if constexpr (GDB) {
+      if (a.tangent == 2) { didx = (long long)(m % a.drow_mod) * a.N + nn; in.v2 = __ldg(a.Zmask + idx); }
+    }
+    in.v0 = __ldg(a.D + didx);
+    if (a.nxt_hi) in.v1 = __ldg(a.Cz_next + idx);
+  } else if (a.mode == 3) {
+    in.v0 = __ldg(a.bias + nn);
+  } else if (a.mode == 1) {
+    if (nn < a.N0) {
+      const long long idx = (long long)m * a.N0 + nn;
+      in.v0 = __ldg(a.Zprev + idx);
+      in.v1 = __ldg(a.Cz + idx);
+      if constexpr (GDB) {
+        if (a.dCz) { in.v2 = __ldg(a.Ztprev + idx); in.v3 = a.dCz[idx]; }
+        if (a.Dacc) in.v4 = a.Dacc[idx];
+      }
+    } else {
+      const int e = nn - a.N0;
+      in.v0 = __ldg(a.Cy + (long long)m * a.n + e);
+      in.v1 = grow[e];
+    }
+  }
+  return in;
+}
+
+// the mode's arithmetic on the accumulated product acc and the element's inputs, and the stores
+template <bool GDB>
+__device__ __forceinline__ void tc_epi_apply(const TcArgs& a, int m, int nn, float acc, const TcEpiIn<GDB>& in,
+                                             float* grow) {
+  if (a.mode == 0) {
+    const long long idx = (long long)m * a.N + nn;
+    const float x = acc + in.v0;
+    float z = x > 0.f ? x : a.alpha * x;
+    if constexpr (GDB) {
+      if (a.tangent == 1) z = (in.v0 > 0.f ? 1.f : a.alpha) * acc;
+      else if (a.tangent == 2) z = (in.v2 > 0.f ? 1.f : a.alpha) * x;
+    }
+    a.Z[idx] = z;
+    if (a.nxt_hi) {
+      const float p = z * in.v1;
+      const float h = tf32_hi(p);
+      a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
+      a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
+    }
+  } else if (a.mode == 1) {
+    if (nn < a.N0) {
+      const float da = in.v0 > 0.f ? 1.f : a.alpha;
+      const float p = da * in.v1 * acc;
+      const float h = tf32_hi(p);
+      a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
+      a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
+      if constexpr (GDB) {
+        const long long idx = (long long)m * a.N0 + nn;
+        if (a.dprev_plain) a.dprev_plain[idx] = p;
+        if (a.acc_plain) a.acc_plain[idx] = acc;
+        if (a.dCz) a.dCz[idx] = fmaf(a.kappa * in.v2, acc, in.v3);
+        if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, in.v4);
+      }
+    } else {
+      const int e = nn - a.N0;
+      grow[e] = fmaf(a.g_scale * in.v0, acc, in.v1);
+    }
+  } else if (a.mode == 3) {
+    int r = 0;
+#pragma unroll
+    for (int t = 1; t < 4; ++t) if (t < a.nr && nn >= a.rbeg[t]) r = t;
+    float v = acc + in.v0;
+    if (a.rrelu[r]) v = fmaxf(v, 0.f);
+    const int c = nn - a.rbeg[r];
+    if (r == 0 && a.r0_hi) {
+      const float h = tf32_hi(v);
+      a.r0_hi[(long long)m * a.rld[0] + c] = h;
+      a.r0_lo[(long long)m * a.rld[0] + c] = tf32_lo(v, h);
+    } else {
+      a.rdst[r][(long long)m * a.rld[r] + c] = v;
+    }
+  } else {
+    a.C[(long long)m * a.N + nn] = acc;
+  }
+}
+
 // <128,3>: one CTA / SM (194 KB);  <64,4>: one CTA / SM, deeper ring for small grids;
 // <64,2>: two CTAs / SM (98 KB each) so that one CTA's epilogue overlaps the other's main loop.
 template <int BN, int NST_, bool GDB = false>
@@ -308,54 +411,14 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     for (int rr = rlo + warp; rr < rhi; rr += TC_CONSUMER_WARPS) {   // this warp's rows of the CTA's row slice
       const int m = m0 + rr;
       if (m >= a.M) break;
-      float* grow = nullptr;
-      if (a.mode == 1)
-        grow = (a.perm == nullptr) ? a.g + (long long)m * a.g_row_stride
-                                   : a.g + ((long long)m * a.KS + a.perm[(long long)m * a.KS + a.count[m]]) * a.n;
+      float* grow = a.mode == 1 ? tc_g_row(a, m) : nullptr;
       for (int c = lane; c < BN; c += 32) {
         const int nn = n0 + c;
         if (nn >= a.N) break;
         float acc = 0.f;
         for (int qq = 0; qq < S; ++qq) acc += *cl.map_shared_rank(P + rr * PP + c, qq);
-        if (a.mode == 0) {
-          const long long idx = (long long)m * a.N + nn;
-          float dv;
-          if (GDB && a.tangent == 2) dv = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
-          else dv = __ldg(a.D + idx);
-          const float x = acc + dv;
-          float z = x > 0.f ? x : a.alpha * x;
-          if constexpr (GDB) {
-            if (a.tangent == 1) z = (dv > 0.f ? 1.f : a.alpha) * acc;
-            else if (a.tangent == 2) z = (__ldg(a.Zmask + idx) > 0.f ? 1.f : a.alpha) * x;
-          }
-          a.Z[idx] = z;
-          if (a.nxt_hi) {
-            const float p = z * __ldg(a.Cz_next + idx);
-            const float h = tf32_hi(p);
-            a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
-            a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
-          }
-        } else if (a.mode == 2) {
-          a.C[(long long)m * a.N + nn] = acc;
-        } else if (a.mode == 1) {   // (mode 3 never launches split: launch_tc_gemm)
-          if (nn < a.N0) {
-            const long long idx = (long long)m * a.N0 + nn;
-            const float da = __ldg(a.Zprev + idx) > 0.f ? 1.f : a.alpha;
-            const float p = da * __ldg(a.Cz + idx) * acc;
-            const float h = tf32_hi(p);
-            a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
-            a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
-            if constexpr (GDB) {
-              if (a.dprev_plain) a.dprev_plain[idx] = p;
-              if (a.acc_plain) a.acc_plain[idx] = acc;
-              if (a.dCz) a.dCz[idx] = fmaf(a.kappa * __ldg(a.Ztprev + idx), acc, a.dCz[idx]);
-              if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, a.Dacc[idx]);
-            }
-          } else {
-            const int e = nn - a.N0;
-            grow[e] = fmaf(a.g_scale * __ldg(a.Cy + (long long)m * a.n + e), acc, grow[e]);
-          }
-        }
+        if (a.mode != 3)   // (mode 3 never launches split: launch_tc_gemm)
+          tc_epi_apply<GDB>(a, m, nn, acc, tc_epi_load<GDB>(a, m, nn, grow), grow);
       }
     }
     cg::this_cluster().sync();   // partial tiles stay alive until every rank has read them
@@ -366,11 +429,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
   unsigned long long growp = 0;
   if (a.mode == 1 && lane < 16) {
     const int mr = m0 + warp * 16 + lane;
-    if (mr < a.M) {
-      float* gp = (a.perm == nullptr) ? a.g + (long long)mr * a.g_row_stride
-                                      : a.g + ((long long)mr * a.KS + a.perm[(long long)mr * a.KS + a.count[mr]]) * a.n;
-      growp = reinterpret_cast<unsigned long long>(gp);
-    }
+    if (mr < a.M) growp = reinterpret_cast<unsigned long long>(tc_g_row(a, mr));
   }
 #pragma unroll
   for (int c0 = 0; c0 < BN; c0 += 32) {
@@ -382,98 +441,21 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     constexpr int RG = 8;
     for (int r0 = 0; r0 < 16; r0 += RG) {
       if (m0 + warp * 16 + r0 >= a.M) break;           // warp-uniform
-      float acc[RG], in0[RG], in1[RG];
-      float in2[GDB ? RG : 1], in3[GDB ? RG : 1], in4[GDB ? RG : 1];
-      unsigned long long gp[RG];
+      float acc[RG];
+      TcEpiIn<GDB> in[RG];
+      float* gp[RG];
 #pragma unroll
       for (int i = 0; i < RG; ++i) {
         const int m = m0 + warp * 16 + r0 + i;
         acc[i] = P[(warp * 16 + r0 + i) * PP + c0 + lane];
-        gp[i] = __shfl_sync(0xffffffffu, growp, r0 + i);
-        in0[i] = 0.f; in1[i] = 0.f;
-        if (nv && m < a.M) {
-          if (a.mode == 0) {
-            const long long idx = (long long)m * a.N + nn;
-            if (GDB && a.tangent == 2) {
-              in0[i] = __ldg(a.D + (long long)(m % a.drow_mod) * a.N + nn);
-              in1[i] = __ldg(a.Zmask + idx);
-            } else {
-              in0[i] = __ldg(a.D + idx);
-              if (a.nxt_hi) in1[i] = __ldg(a.Cz_next + idx);
-            }
-          } else if (a.mode == 3) {
-            in0[i] = __ldg(a.bias + nn);
-          } else if (a.mode == 1) {
-            if (nn < a.N0) {
-              const long long idx = (long long)m * a.N0 + nn;
-              in0[i] = __ldg(a.Zprev + idx);
-              in1[i] = __ldg(a.Cz + idx);
-              if constexpr (GDB) {
-                if (a.dCz) { in2[i] = __ldg(a.Ztprev + idx); in3[i] = a.dCz[idx]; }
-                if (a.Dacc) in4[i] = a.Dacc[idx];
-              }
-            } else {
-              const int e = nn - a.N0;
-              in0[i] = __ldg(a.Cy + (long long)m * a.n + e);
-              in1[i] = reinterpret_cast<const float*>(gp[i])[e];
-            }
-          }
-        }
+        gp[i] = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, growp, r0 + i));
+        if (nv && m < a.M) in[i] = tc_epi_load<GDB>(a, m, nn, gp[i]);
       }
 #pragma unroll
       for (int i = 0; i < RG; ++i) {
         const int m = m0 + warp * 16 + r0 + i;
         if (!nv || m >= a.M) continue;
-        if (a.mode == 0) {
-          const long long idx = (long long)m * a.N + nn;
-          const float x = acc[i] + in0[i];
-          float z = x > 0.f ? x : a.alpha * x;
-          if constexpr (GDB) {
-            if (a.tangent == 1) z = (in0[i] > 0.f ? 1.f : a.alpha) * acc[i];
-            else if (a.tangent == 2) z = (in1[i] > 0.f ? 1.f : a.alpha) * x;
-          }
-          a.Z[idx] = z;
-          if (a.nxt_hi) {
-            const float p = z * in1[i];
-            const float h = tf32_hi(p);
-            a.nxt_hi[(long long)m * a.nxt_ld + nn] = h;
-            a.nxt_lo[(long long)m * a.nxt_ld + nn] = tf32_lo(p, h);
-          }
-        } else if (a.mode == 1) {
-          if (nn < a.N0) {
-            const float da = in0[i] > 0.f ? 1.f : a.alpha;
-            const float p = da * in1[i] * acc[i];
-            const float h = tf32_hi(p);
-            a.dprev_hi[(long long)m * a.dprev_ld + nn] = h;
-            a.dprev_lo[(long long)m * a.dprev_ld + nn] = tf32_lo(p, h);
-            if constexpr (GDB) {
-              const long long idx = (long long)m * a.N0 + nn;
-              if (a.dprev_plain) a.dprev_plain[idx] = p;
-              if (a.acc_plain) a.acc_plain[idx] = acc[i];
-              if (a.dCz) a.dCz[idx] = fmaf(a.kappa * in2[i], acc[i], in3[i]);
-              if (a.Dacc) a.Dacc[idx] = fmaf(a.kappa, p, in4[i]);
-            }
-          } else {
-            const int e = nn - a.N0;
-            reinterpret_cast<float*>(gp[i])[e] = fmaf(a.g_scale * in0[i], acc[i], in1[i]);
-          }
-        } else if (a.mode == 3) {
-          int r = 0;
-#pragma unroll
-          for (int t = 1; t < 4; ++t) if (t < a.nr && nn >= a.rbeg[t]) r = t;
-          float v = acc[i] + in0[i];
-          if (a.rrelu[r]) v = fmaxf(v, 0.f);
-          const int c = nn - a.rbeg[r];
-          if (r == 0 && a.r0_hi) {
-            const float h = tf32_hi(v);
-            a.r0_hi[(long long)m * a.rld[0] + c] = h;
-            a.r0_lo[(long long)m * a.rld[0] + c] = tf32_lo(v, h);
-          } else {
-            a.rdst[r][(long long)m * a.rld[r] + c] = v;
-          }
-        } else {
-          a.C[(long long)m * a.N + nn] = acc[i];
-        }
+        tc_epi_apply<GDB>(a, m, nn, acc[i], in[i], gp[i]);
       }
     }
   }
@@ -656,8 +638,8 @@ int launch_tc_gemm(const float* Ah, const float* Al, long long lda, const float*
   if ((rc = make_tmap(&tAl, Al, a.M, a.K, lda, TC_BM))) return rc;
   if ((rc = make_tmap(&tBh, Bh, a.N, a.K, ldb, BN))) return rc;
   if ((rc = make_tmap(&tBl, Bl, a.N, a.K, ldb, BN))) return rc;
-  // split-K over a cluster when the tile grid leaves most of the chip idle (C2: 4 row tiles); only <64,4> and the
-  // modes the split-K epilogue implements (0, 1, 2; the mode-3 gate epilogue never splits)
+  // split-K over a cluster when the tile grid leaves most of the chip idle (C2: 4 row tiles); only <64,4> splits,
+  // and the mode-3 gate GEMM never does
   int splitk = 1;
   if (cfg == 1 && a.mode != 3) {
     const int tiles = cdiv(a.N, 64) * gy, nkb = cdiv(a.K, TC_BK);
@@ -736,10 +718,47 @@ void out_layer_launch(const icnn_picnn* h, const icnn_gates* gt, const float* Zl
                       const int* perm, const int* count, int KS, const int* skip, cudaStream_t st);
 size_t picnn_simt_ws_floats(const icnn_picnn* h, int B, size_t* zoff, size_t* doff);
 
+// (sc y + sh) o cy_i for every hidden layer, straight into the K-concatenated operands hi[i] / lo[i]
+static void gate_y_launch(const icnn_picnn* h, const icnn_gates* gt, const float* y, float sc, float sh,
+                          float* const* hi, float* const* lo, const int* skip, cudaStream_t st) {
+  GateYArgs ga{};
+  ga.B = gt->B; ga.n = h->n; ga.L = h->L; ga.y = y; ga.sc = sc; ga.sh = sh; ga.skip_if_zero = skip;
+  for (int i = 0; i < h->L; ++i) {
+    ga.cy[i] = gt->cy[i]; ga.hi[i] = hi[i]; ga.lo[i] = lo[i]; ga.ld[i] = ld4(h->prev(i) + h->n); ga.off[i] = h->prev(i);
+  }
+  const long long N = (long long)gt->B * h->n;
+  gate_y_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(ga);
+}
+
+// forward GEMM of hidden layer i: Z_i = act(A'_i Wcat_i + d_i) into Z and, below the last hidden layer, the next
+// operand's columns A'_{i+1}[:, 0:s_i] = Z_i o cz_{i+1} into nxt_hi[i + 1] / nxt_lo[i + 1]
+static TcArgs fwd_layer_args(const icnn_picnn* h, const icnn_gates* gt, int i, float* Z, float* const* nxt_hi,
+                             float* const* nxt_lo) {
+  TcArgs a{};
+  a.M = gt->B; a.N = h->hidden[i]; a.K = h->prev(i) + h->n; a.mode = 0;
+  a.D = gt->d[i]; a.Z = Z; a.alpha = h->alpha;
+  if (i + 1 < h->L) {
+    a.Cz_next = gt->cz[i + 1]; a.nxt_hi = nxt_hi[i + 1]; a.nxt_lo = nxt_lo[i + 1]; a.nxt_ld = ld4(h->hidden[i] + h->n);
+  }
+  return a;
+}
+
+// backward GEMM of hidden layer i: delta_i Wcat_i^T -> delta_{i-1} = act'(Z_{i-1}) o cz_i o (.) into dprev_hi /
+// dprev_lo, and g += cy_i o (.) into the rows of g at g_row_stride (g_scale 1)
+static TcArgs bwd_layer_args(const icnn_picnn* h, const icnn_gates* gt, int i, float* const* Z, float* dprev_hi,
+                             float* dprev_lo, float* g, long long g_row_stride) {
+  TcArgs a{};
+  a.M = gt->B; a.N0 = h->prev(i); a.N = a.N0 + h->n; a.K = h->hidden[i]; a.mode = 1; a.alpha = h->alpha;
+  a.Zprev = i ? Z[i - 1] : nullptr; a.Cz = i ? gt->cz[i] : nullptr;
+  a.dprev_hi = dprev_hi; a.dprev_lo = dprev_lo; a.dprev_ld = ld4(a.N0);
+  a.Cy = gt->cy[i]; a.g = g; a.g_row_stride = g_row_stride; a.n = h->n; a.g_scale = 1.f;
+  return a;
+}
+
 int picnn_fg_tc(const icnn_picnn* h, const icnn_gates* gt, const float* y32, float* f, float* g,
                 long long g_row_stride, const int* perm, const int* count, int KS, void* workspace,
                 const int* skip, cudaStream_t st) {
-  const int B = gt->B, n = h->n, L = h->L;
+  const int B = gt->B, L = h->L;
   size_t zoff[ICNN_MAX_LAYERS], sdoff[2], aoff[2 * ICNN_MAX_LAYERS], doff[4];
   const size_t simt = picnn_simt_ws_floats(h, B, zoff, sdoff);
   picnn_tc_ws_floats(h, B, aoff, doff);
@@ -751,29 +770,18 @@ int picnn_fg_tc(const icnn_picnn* h, const icnn_gates* gt, const float* y32, flo
   float* dh[2] = {tcw + doff[0], tcw + doff[2]};
   float* dl[2] = {tcw + doff[1], tcw + doff[3]};
 
-  {  // (s y + t) o cy_i for every hidden layer, straight into the K-concatenated operands
-    GateYArgs ga{};
-    ga.B = B; ga.n = n; ga.L = L; ga.y = y32; ga.sc = gt->in_scale; ga.sh = gt->in_shift; ga.skip_if_zero = skip;
-    for (int i = 0; i < L; ++i) { ga.cy[i] = gt->cy[i]; ga.hi[i] = Ah[i]; ga.lo[i] = Al[i]; ga.ld[i] = ld4(h->prev(i) + n); ga.off[i] = h->prev(i); }
-    const long long N = (long long)B * n;
-    gate_y_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(ga);
-  }
+  gate_y_launch(h, gt, y32, gt->in_scale, gt->in_shift, Ah, Al, skip, st);
   for (int i = 0; i < L; ++i) {
-    TcArgs a{};
-    a.M = B; a.N = h->hidden[i]; a.K = h->prev(i) + n; a.mode = 0;
-    a.D = gt->d[i]; a.Z = Z[i]; a.alpha = h->alpha; a.skip_if_zero = skip;
-    if (i + 1 < L) { a.Cz_next = gt->cz[i + 1]; a.nxt_hi = Ah[i + 1]; a.nxt_lo = Al[i + 1]; a.nxt_ld = ld4(h->hidden[i] + n); }
+    TcArgs a = fwd_layer_args(h, gt, i, Z[i], Ah, Al);
+    a.skip_if_zero = skip;
     int rc = launch_tc_gemm(Ah[i], Al[i], ld4(a.K), h->Wf_hi[i], h->Wf_lo[i], ld4(a.K), a, st);
     if (rc) return rc;
   }
   out_layer_launch(h, gt, Z[L - 1], y32, f, nullptr, dh[0], dl[0], g, g_row_stride, perm, count, KS, skip, st);
   int cur = 0;
   for (int i = L - 1; i >= 0; --i) {
-    TcArgs a{};
-    a.M = B; a.N0 = h->prev(i); a.N = a.N0 + n; a.K = h->hidden[i]; a.mode = 1; a.alpha = h->alpha;
-    a.Zprev = i ? Z[i - 1] : nullptr; a.Cz = i ? gt->cz[i] : nullptr; a.dprev_hi = dh[cur ^ 1]; a.dprev_lo = dl[cur ^ 1]; a.dprev_ld = ld4(a.N0);
-    a.Cy = gt->cy[i]; a.g = g; a.g_row_stride = g_row_stride; a.perm = perm; a.count = count; a.KS = KS; a.n = n;
-    a.g_scale = gt->g_scale; a.skip_if_zero = skip;
+    TcArgs a = bwd_layer_args(h, gt, i, Z, dh[cur ^ 1], dl[cur ^ 1], g, g_row_stride);
+    a.perm = perm; a.count = count; a.KS = KS; a.g_scale = gt->g_scale; a.skip_if_zero = skip;
     int rc = launch_tc_gemm(dh[cur], dl[cur], ld4(a.K), h->Wb_hi[i], h->Wb_lo[i], ld4(a.K), a, st);
     if (rc) return rc;
     cur ^= 1;
@@ -801,31 +809,17 @@ size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* b
   return off;
 }
 
-static void gdb_gate(const icnn_picnn* h, const icnn_gates* gt, const float* v, float* const* hi, float* const* lo,
-                     cudaStream_t st) {
-  GateYArgs ga{};
-  ga.B = gt->B; ga.n = h->n; ga.L = h->L; ga.y = v; ga.sc = 1.f; ga.sh = 0.f; ga.skip_if_zero = nullptr;
-  for (int i = 0; i < h->L; ++i) {
-    ga.cy[i] = gt->cy[i]; ga.hi[i] = hi[i]; ga.lo[i] = lo[i]; ga.ld[i] = ld4(h->prev(i) + h->n); ga.off[i] = h->prev(i);
-  }
-  const long long N = (long long)gt->B * h->n;
-  gate_y_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(ga);
-}
-
 // the (a o cy_i) columns of the tangent operands: constant over the GD iterations
 void picnn_gdb_tc_gate_a(const icnn_picnn* h, const icnn_gates* gt, const float* a, const GdbTcBufs& b, cudaStream_t st) {
-  gdb_gate(h, gt, a, b.Ath, b.Atl, st);
+  gate_y_launch(h, gt, a, 1.f, 0.f, b.Ath, b.Atl, nullptr, st);
 }
 
 // primal forward of every hidden layer at b.y (and, with tangent, the tangent layers on direction a)
 int picnn_gdb_tc_forward(const icnn_picnn* h, const icnn_gates* gt, const GdbTcBufs& b, bool tangent, cudaStream_t st) {
-  const int B = gt->B, n = h->n, L = h->L;
-  gdb_gate(h, gt, b.y, b.Ah, b.Al, st);
+  const int L = h->L;
+  gate_y_launch(h, gt, b.y, 1.f, 0.f, b.Ah, b.Al, nullptr, st);
   for (int i = 0; i < L; ++i) {
-    TcArgs a{};
-    a.M = B; a.N = h->hidden[i]; a.K = h->prev(i) + n; a.mode = 0;
-    a.D = gt->d[i]; a.Z = b.Z[i]; a.alpha = h->alpha;
-    if (i + 1 < L) { a.Cz_next = gt->cz[i + 1]; a.nxt_hi = b.Ah[i + 1]; a.nxt_lo = b.Al[i + 1]; a.nxt_ld = ld4(h->hidden[i] + n); }
+    TcArgs a = fwd_layer_args(h, gt, i, b.Z[i], b.Ah, b.Al);
     int rc = launch_tc_gemm(b.Ah[i], b.Al[i], ld4(a.K), h->Wf_hi[i], h->Wf_lo[i], ld4(a.K), a, st, true);
     if (rc) return rc;
     if (tangent) {
@@ -842,11 +836,7 @@ int picnn_gdb_tc_forward(const icnn_picnn* h, const icnn_gates* gt, const GdbTcB
 // plain) and g; the optional accumulations / plain stores of GdbTcBufs run in the epilogue
 int picnn_gdb_tc_backward_layer(const icnn_picnn* h, const icnn_gates* gt, const GdbTcBufs& b, int i, int cur,
                                 cudaStream_t st) {
-  TcArgs a{};
-  a.M = gt->B; a.N0 = h->prev(i); a.N = a.N0 + h->n; a.K = h->hidden[i]; a.mode = 1; a.alpha = h->alpha;
-  a.Zprev = i ? b.Z[i - 1] : nullptr; a.Cz = i ? gt->cz[i] : nullptr;
-  a.dprev_hi = b.dh[cur ^ 1]; a.dprev_lo = b.dl[cur ^ 1]; a.dprev_ld = ld4(a.N0);
-  a.Cy = gt->cy[i]; a.g = b.g; a.g_row_stride = h->n; a.n = h->n; a.g_scale = 1.f;
+  TcArgs a = bwd_layer_args(h, gt, i, b.Z, b.dh[cur ^ 1], b.dl[cur ^ 1], b.g, h->n);
   if (i > 0) {
     if (b.want_plain) a.dprev_plain = b.dstore[i - 1] ? b.dstore[i - 1] : b.dp[cur ^ 1];
     a.acc_plain = b.astore[i];

@@ -1,4 +1,5 @@
-// The 3xTF32 wgmma GEMM of picnn_tc.cu as seen by the other translation units that launch it (conv_picnn.cu):
+// The 3xTF32 wgmma GEMM of picnn_tc.cu as seen by the other translation units that launch it (conv_picnn.cu,
+// conv_train_grad.cu):
 //   C[M,N] = A[M,K] * B[N,K]^T, both operands K-major, pre-split TF32 hi/lo, row pitches multiples of 4 floats,
 // with the fused epilogues selected by TcArgs::mode.
 #pragma once
@@ -9,7 +10,7 @@ namespace icnn {
 struct TcArgs {
   int M, N, K;
   int ch;    // half k-blocks per accumulation chunk (>= 1), set by launch_tc_gemm
-  int mode;  // 0 forward, 1 backward, 2 plain store (self test)
+  int mode;  // 0 forward, 1 backward, 2 plain store C = acc, 3 x-path gates
   // forward epilogue: Z = act(acc + D); optional next-layer operand A'_{next}[:, 0:N] = Z o Cz_next (hi/lo)
   const float* D; float* Z; float alpha;
   const float* Cz_next; float* nxt_hi; float* nxt_lo; int nxt_ld;
@@ -17,8 +18,9 @@ struct TcArgs {
   int N0; const float* Zprev; const float* Cz; float* dprev_hi; float* dprev_lo; int dprev_ld;
   const float* Cy; float* g; long long g_row_stride; const int* perm; const int* count; int KS; int n;
   float g_scale;
-  float* C;  // mode 2
-  // GD training backward (GDB instantiation only, gd_backward.cu):
+  float* C;  // mode 2: the self test and the conv PICNN's plain GEMMs (conv_picnn.cu, conv_train_grad.cu)
+  // training gradients (GDB instantiation only): the GD training backward (gd_backward.cu) and the bundle-entropy
+  // gradient (train_grad.cu) through picnn_tc.cu's GDB layer GEMMs; conv_train_grad.cu launches with tangent = 1:
   //   mode 0 with tangent != 0: Z = act'(D) o acc (D holds the primal activation), no bias
   //   mode 1: optional plain copy of delta_prev, dCz += kappa * Ztprev o acc, Dacc += kappa * delta_prev
   //   mode 0 with tangent == 2 (stored-pattern phase): Z = act'(Zmask) o (acc + D[(row % drow_mod), :])
