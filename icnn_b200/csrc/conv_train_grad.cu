@@ -27,9 +27,10 @@
 // float64 a different cut only reorders additions, and the results agree up to the final rounding.
 // The per-sample outputs are float64 sums over a sample's rows, rounded once per chunk: only a sample with more rows
 // than a chunk holds (split over chunks, as in train_grad.cu) sees more than one rounding.
-// A conv layer's reduction is long (rows H_{l+1} W_{l+1}) and its output small (K_l x C_l), so the reduction is
-// split over the rows into enough CTAs to fill the machine (wsplit_kernel), and the float64 partials are summed in
-// a fixed order (ws_reduce_kernel): no atomics, the same result on every call.
+// The weight gradients are wgrad.cuh's GEMM in float64 with delta's TF32 hi/lo pair as D + Dlo.  A conv layer's
+// reduction is long (rows H_{l+1} W_{l+1}) and its output small (K_l x C_l), so wgrad_parts splits it over the rows
+// into enough CTAs to fill the machine and the float64 partials are summed in a fixed order: no atomics, the same
+// result on every call.
 //
 // The GD training backward of the same net (icnn_conv_gd_backward, completion/icnn.back.py:133-156) is this gradient
 // on other rows: with a = dloss/dy_N and kappa_i of gd_backward.cu's derivation (the conv energy is piecewise linear
@@ -39,6 +40,7 @@
 #include "conv_picnn.cuh"
 #include "gdb.cuh"
 #include "train_rows.cuh"
+#include "wgrad.cuh"
 
 #include <vector>
 
@@ -86,79 +88,6 @@ static __global__ void im2col_plain_kernel(const float* Z, const float* cz, cons
   A[i] = v;
 }
 
-// Split-over-rows float64 weight gradient.  CTA (x, y, z) owns the 64 x 64 output tile (kk0 = 64 y, o0 = 64 x) and
-// the rows [M z / P, M (z+1) / P):
-//   part[z][kk, o] = sum_m A[m, kk] G[m, kk] (Dh + Dl)[m, o]      (G == nullptr: 1; Dh == nullptr: a column of ones)
-// Dh + Dl is the TF32 hi/lo pair of delta (exact in float32).
-struct WsArgs {
-  int M, K, N, P;
-  const float* A; const float* G; int lda;
-  const float* Dh; const float* Dl; int ldd;
-  double* part;
-};
-
-static __global__ void __launch_bounds__(256) wsplit_kernel(WsArgs a) {
-  __shared__ __align__(16) float As[16][64 + 4];
-  __shared__ __align__(16) float Ds[16][64 + 4];
-  const int t = threadIdx.x, ty = t / 16, tx = t % 16, lk = t / 16, lc = (t % 16) * 4;
-  const int k0 = blockIdx.y * 64, n0 = blockIdx.x * 64, z = blockIdx.z;
-  const long long mb = (long long)a.M * z / a.P, me = (long long)a.M * (z + 1) / a.P;
-  double acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0;
-  for (long long m0 = mb; m0 < me; m0 += 16) {
-    const long long m = m0 + lk;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int kk = k0 + lc + i, o = n0 + lc + i;
-      float va = 0.f, vd = 0.f;
-      if (m < me) {
-        if (kk < a.K) {
-          va = a.A[m * a.lda + kk];
-          if (a.G) va *= a.G[m * a.lda + kk];
-        }
-        if (o < a.N) vd = a.Dh ? a.Dh[m * a.ldd + o] + a.Dl[m * a.ldd + o] : 1.f;
-      }
-      As[lk][lc + i] = va;
-      Ds[lk][lc + i] = vd;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      const float4 av = *reinterpret_cast<const float4*>(&As[k][ty * 4]);
-      const float4 dv = *reinterpret_cast<const float4*>(&Ds[k][tx * 4]);
-      const double aa[4] = {av.x, av.y, av.z, av.w}, dd[4] = {dv.x, dv.y, dv.z, dv.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fma(aa[i], dd[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  double* pz = a.part + (long long)z * a.K * a.N;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int kk = k0 + ty * 4 + i;
-    if (kk >= a.K) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int o = n0 + tx * 4 + j;
-      if (o < a.N) pz[(long long)kk * a.N + o] = acc[i][j];
-    }
-  }
-}
-
-// acc[i] += sum over z = 0..P-1 of part[z][i], in that order
-static __global__ void ws_reduce_kernel(double* acc, const double* part, int P, long long N) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  double s = 0.0;
-  for (int z = 0; z < P; ++z) s += part[(long long)z * N + i];
-  acc[i] += s;
-}
-
 // y_red gradients of conv layer g from the rows' rhat_l [rows, Hi Wi] and rho_{l+1} [rows, Ho Wo]; CTA (t, z) sums
 // the output pixels [Mo z / P, Mo (z+1) / P) into part[z][t]:
 //   t < k^2: rhat_l[in(o, t)] rho_{l+1}[o] (0 in the padding);  t = k^2: c_row rho_{l+1}[o]
@@ -204,7 +133,7 @@ static __global__ void conv_unpack_kernel(const double* acc, int taps, int Cp, i
 // ---- workspace --------------------------------------------------------------------------------------------------
 struct CtgLayout {
   size_t off, row_u, acc64, part64, fl;   // bytes
-  size_t n64, npart;                      // doubles
+  size_t n64;                             // doubles
   size_t aw[2 * ICNN_MAX_LAYERS], ared[ICNN_MAX_LAYERS];   // doubles into acc64: dWcat_l / dWz_i, y_red l
   // floats from fl: conv_fg's workspace, per-row gates, e_l, tangents, dense e_z, f and g scratch
   size_t cws, cy[2 * ICNN_MAX_LAYERS], cz[2 * ICNN_MAX_LAYERS], d[2 * ICNN_MAX_LAYERS], e[ICNN_MAX_LAYERS];
@@ -213,17 +142,6 @@ struct CtgLayout {
   size_t total;
 };
 
-// CTAs of the split reduction of an [M] x [K, N] weight gradient: enough to fill the machine twice over, at least
-// 256 reduction rows each
-static int ws_parts(long long M, int K, int N) {
-  const long long tiles = (long long)cdiv(N, 64) * cdiv(K, 64);
-  long long p = (2LL * device_sms() + tiles - 1) / tiles;
-  const long long pm = (M + 255) / 256;
-  if (p > pm) p = pm;
-  if (p < 1) p = 1;
-  if (p > 1024) p = 1024;
-  return (int)p;
-}
 static int yred_parts(long long Mo) {
   const long long p = (Mo + 4095) / 4096;
   return (int)(p < 1 ? 1 : p > 64 ? 64 : p);
@@ -266,26 +184,18 @@ static CtgLayout ctg_layout(const icnn_conv_picnn* h, int B, long long R) {
     const double per_row = 4.0 * (double)(conv_ws_floats(h, (int)probe, nullptr, &w) + ctg_floats(h, probe, nullptr)) / probe;
     t.cap = chunk_rows(per_row, R);
   }
-  size_t n64 = 0, npart = 1;
-  auto part = [&](long long M, int K, int N) {
-    const size_t p = (size_t)ws_parts(M, K, N) * K * N;
-    npart = p > npart ? p : npart;
-  };
+  size_t n64 = 0, npart = wgrad_part_bytes() / sizeof(double);   // the y_red partials share the region
   for (int l = 0; l < h->Lc; ++l) {
     const ConvGeom& g = h->g[l];
     t.aw[l] = n64; n64 += (size_t)g.K * g.C;
-    part(t.cap * g.Ho * g.Wo, g.K, g.C);
     if (l + 1 < h->Lc) {
       t.ared[l] = n64; n64 += (size_t)g.k * g.k + 1;
       const size_t p = (size_t)yred_parts(t.cap * g.Ho * g.Wo) * (g.k * g.k + 1);
       npart = p > npart ? p : npart;
     }
   }
-  for (int j = 0; j < h->Ld; ++j) {
-    t.aw[h->Lc + j] = n64; n64 += (size_t)h->in_w(j) * h->fcs[j];
-    part(t.cap, h->in_w(j), h->fcs[j]);
-  }
-  t.n64 = n64; t.npart = npart;
+  for (int j = 0; j < h->Ld; ++j) { t.aw[h->Lc + j] = n64; n64 += (size_t)h->in_w(j) * h->fcs[j]; }
+  t.n64 = n64;
   size_t bytes = 0;
   t.off = bytes; bytes += al(sizeof(long long) * ((size_t)B + 1));
   t.row_u = bytes; bytes += al(sizeof(int) * (size_t)t.cap);
@@ -314,16 +224,6 @@ static CtgLayout ctg_layout(const icnn_conv_picnn* h, int B, long long R) {
     cudaError_t _le = cudaGetLastError();                                                               \
     if (_le != cudaSuccess) { set_error("conv_train_grad %s: %s", what, cudaGetErrorString(_le)); return ICNN_E_CUDA; } \
   } while (0)
-
-// part = split reduction of a.{M, K, N}, then acc += its fixed-order sum
-static int wgrad_split(WsArgs a, double* acc, cudaStream_t st) {
-  a.P = ws_parts(a.M, a.K, a.N);
-  wsplit_kernel<<<dim3(cdiv(a.N, 64), cdiv(a.K, 64), a.P), 256, 0, st>>>(a);
-  const long long KN = (long long)a.K * a.N;
-  ws_reduce_kernel<<<nb(KN), 256, 0, st>>>(acc, a.part, a.P, KN);
-  CTG_LAUNCH("weight gradient");
-  return ICNN_OK;
-}
 
 // every per-layer buffer of icnn_conv_train_grads the layers use is given
 static int ctg_check_buffers(const icnn_conv_picnn* h, const icnn_conv_train_grads* gr) {
@@ -514,23 +414,29 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
         const ConvGeom& G = h->g[l];
         const long long M = (long long)rows * G.Ho * G.Wo;
         im2col_plain_kernel<<<nb(M * G.K), 256, 0, st>>>(l ? zt[l - 1] : nullptr, cz[l], rt[l], cy[l], G, rows, w.Ah[l]);
-        WsArgs a{};
-        a.M = (int)M; a.K = G.K; a.N = G.C; a.A = w.Ah[l]; a.lda = G.K;
-        a.Dh = w.dh[l]; a.Dl = w.dl[l]; a.ldd = ld4(G.C); a.part = part64;
-        if ((rc = wgrad_split(a, acc64 + t.aw[l], st))) return rc;
-        if (l + 1 < Lc) {
-          const int P = yred_parts(M), T1 = G.k * G.k + 1;
-          yred_grad_kernel<<<dim3(T1, P), 256, 0, st>>>(rt[l], w.rho[l + 1], cc, G, M, part64);
-          ws_reduce_kernel<<<nb(T1), 256, 0, st>>>(acc64 + t.ared[l], part64, P, T1);
+        WgradArgs a{};
+        a.M = G.K; a.N = G.C; a.Kb = (int)M; a.A = w.Ah[l]; a.lda = G.K;
+        a.D = w.dh[l]; a.Dlo = w.dl[l]; a.ldd = ld4(G.C); a.C64 = acc64 + t.aw[l]; a.ldc = G.C; a.kappa = 1.f;
+        a.part = part64;
+        launch_wgrad(a, st);
+        CTG_LAUNCH("weight gradient");
+        if (l + 1 < Lc) {   // acc += the y_red partials in rank order: the reduce of an M = 1 weight gradient
+          WgradArgs r{};
+          r.M = 1; r.N = G.k * G.k + 1; r.C64 = acc64 + t.ared[l]; r.ldc = r.N; r.kappa = 1.f; r.part = part64;
+          const int P = yred_parts(M);
+          yred_grad_kernel<<<dim3(r.N, P), 256, 0, st>>>(rt[l], w.rho[l + 1], cc, G, M, part64);
+          wgrad_reduce_kernel<double><<<nb(r.N), 256, 0, st>>>(r, P);
           CTG_LAUNCH("y_red gradient");
         }
       }
       for (int j = 0; j < Ld; ++j) {
         const int i = Lc + j;
-        WsArgs a{};
-        a.M = rows; a.K = h->in_w(j); a.N = h->fcs[j]; a.A = zt[i - 1]; a.G = cz[i]; a.lda = a.K; a.part = part64;
-        if (j + 1 < Ld) { a.Dh = w.fdh[j]; a.Dl = w.fdl[j]; a.ldd = ld4(h->fcs[j]); }
-        if ((rc = wgrad_split(a, acc64 + t.aw[i], st))) return rc;
+        WgradArgs a{};
+        a.M = h->in_w(j); a.N = h->fcs[j]; a.Kb = rows; a.A = zt[i - 1]; a.G = cz[i]; a.lda = a.M;
+        if (j + 1 < Ld) { a.D = w.fdh[j]; a.Dlo = w.fdl[j]; a.ldd = ld4(h->fcs[j]); }
+        a.C64 = acc64 + t.aw[i]; a.ldc = a.N; a.kappa = 1.f; a.part = part64;
+        launch_wgrad(a, st);
+        CTG_LAUNCH("weight gradient");
       }
 
       // ---- per-sample gate adjoints ----

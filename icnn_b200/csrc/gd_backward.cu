@@ -26,10 +26,11 @@
 // deterministic loop (bit-identical iterates) with, per iteration, the tangent forward (the same
 // gated product with the activation pattern of the primal Z_l), the dcz / Delta accumulation fused
 // into the backward epilogue, and one weight-gradient GEMM per Wz_l.
-// wgrad_gemm_kernel: FP32 FFMA, reduction over the batch split over a thread-block cluster and
-// summed through distributed shared memory -- no atomics, deterministic.
+// The weight-gradient GEMMs are wgrad.cuh's (FP32 FFMA, rows split over CTAs and the parts summed in a
+// fixed order: no atomics, deterministic); their partial tiles go to GdbLayout::wpart.
 #include "gated_gemm.cuh"
 #include "gdb.cuh"
+#include "wgrad.cuh"
 
 #include <cstdlib>
 #include <vector>
@@ -47,148 +48,6 @@ int picnn_gdb_tc_stored_tangent(const icnn_picnn* h, int l, long long M, int B, 
 void out_layer_launch(const icnn_picnn* h, const icnn_gates* gt, const float* Zlast, const float* y32, float* f,
                       float* delta, float* delta_hi, float* delta_lo, float* g, long long g_row_stride,
                       const int* perm, const int* count, int KS, const int* skip, cudaStream_t st);
-
-struct WgradArgs {
-  int M, N, Kb;                       // C is [M, N]; reduction over Kb batch rows
-  const float* A; const float* G; int lda;   // A (optionally gated by G) [Kb, lda]
-  const float* D; int ldd;            // D [Kb, ldd]; nullptr = a column of ones (N == 1)
-  float* C; int ldc; float kappa;     // C += kappa * (A o G)^T D
-  double* C64;                        // optional: float64 accumulation, C64 += kappa * (A o G)^T D (C unused)
-};
-
-// C[m, n] += kappa * sum_b A[b, m] G[b, m] D[b, n].  64x64 tile, 16 batch rows per stage; both
-// operands are read along their contiguous dimension.  gridDim.z = S CTAs of one cluster split the
-// batch and reduce their partial tiles through DSMEM (same scheme as gated_gemm_kernel).
-// Acc = double (WgradArgs::C64): every product of two floats is exact in float64 and the sums over the batch and
-// the split are float64, so the result does not depend on how the rows are split over launches (train_grad.cu).
-constexpr int WG_TILE_BYTES = (int)sizeof(float) * (2 * BK * (BM + PAD) + 2 * BK * (BN + PAD));
-template <typename Acc>
-struct WgSmem {
-  static constexpr int PART = (int)sizeof(Acc) * BM * (BN + 1);
-  static constexpr int BYTES = PART > WG_TILE_BYTES ? PART : WG_TILE_BYTES;
-};
-__device__ __forceinline__ float wg_madd(float x, float y, float acc) { return fmaf(x, y, acc); }
-__device__ __forceinline__ double wg_madd(float x, float y, double acc) { return fma((double)x, (double)y, acc); }
-__device__ __forceinline__ void wg_store(const WgradArgs& a, int m, int nn, float v) {
-  float* c = a.C + (long long)m * a.ldc + nn;
-  *c = fmaf(a.kappa, v, *c);
-}
-__device__ __forceinline__ void wg_store(const WgradArgs& a, int m, int nn, double v) {
-  a.C64[(long long)m * a.ldc + nn] += (double)a.kappa * v;
-}
-
-template <typename Acc>
-__global__ void __launch_bounds__(256) wgrad_gemm_kernel(WgradArgs a) {
-  __shared__ __align__(16) unsigned char smem_raw[WgSmem<Acc>::BYTES];
-  float* smem_f = reinterpret_cast<float*>(smem_raw);
-  float (*As)[BK][BM + PAD] = reinterpret_cast<float (*)[BK][BM + PAD]>(smem_f);
-  float (*Bs)[BK][BN + PAD] = reinterpret_cast<float (*)[BK][BN + PAD]>(smem_f + 2 * BK * (BM + PAD));
-  const int t = threadIdx.x;
-  const int S = gridDim.z;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int ty = t / 16, tx = t % 16;
-  const int l_k = t / 16, l_c = (t % 16) * 4;
-
-  float ra[4], rb[4];
-  auto load_tiles = [&](int b0) {
-    const int b = b0 + l_k;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int m = m0 + l_c + i, nn = n0 + l_c + i;
-      float va = 0.f, vb = 0.f;
-      if (b < a.Kb) {
-        if (m < a.M) {
-          va = a.A[(long long)b * a.lda + m];
-          if (a.G) va *= a.G[(long long)b * a.lda + m];
-        }
-        if (nn < a.N) vb = a.D ? a.D[(long long)b * a.ldd + nn] : 1.f;
-      }
-      ra[i] = va; rb[i] = vb;
-    }
-  };
-  auto store_tiles = [&](int buf) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { As[buf][l_k][l_c + i] = ra[i]; Bs[buf][l_k][l_c + i] = rb[i]; }
-  };
-
-  Acc acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = Acc(0);
-
-  const int nk_all = (a.Kb + BK - 1) / BK;
-  const int kt0 = (int)(((long long)nk_all * blockIdx.z) / S);
-  const int nk = (int)(((long long)nk_all * (blockIdx.z + 1)) / S) - kt0;
-  if (nk > 0) { load_tiles(kt0 * BK); store_tiles(0); }
-  __syncthreads();
-  for (int kt = 0; kt < nk; ++kt) {
-    const int buf = kt & 1;
-    if (kt + 1 < nk) load_tiles((kt0 + kt + 1) * BK);
-#pragma unroll
-    for (int k = 0; k < BK; ++k) {
-      const float4 av = *reinterpret_cast<const float4*>(&As[buf][k][ty * 4]);
-      const float4 bv = *reinterpret_cast<const float4*>(&Bs[buf][k][tx * 4]);
-      const float aa[4] = {av.x, av.y, av.z, av.w};
-      const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = wg_madd(aa[i], bb[j], acc[i][j]);
-    }
-    if (kt + 1 < nk) store_tiles(buf ^ 1);
-    __syncthreads();
-  }
-
-  if (S == 1) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int m = m0 + ty * 4 + i;
-      if (m >= a.M) continue;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int nn = n0 + tx * 4 + j;
-        if (nn < a.N) wg_store(a, m, nn, acc[i][j]);
-      }
-    }
-    return;
-  }
-  cg::cluster_group cluster = cg::this_cluster();
-  Acc (*Ps)[BN + 1] = reinterpret_cast<Acc (*)[BN + 1]>(smem_raw);
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) Ps[ty * 4 + i][tx * 4 + j] = acc[i][j];
-  cluster.sync();
-  const int rank = (int)cluster.block_rank();
-  const int r_lo = (BM * rank) / S, r_hi = (BM * (rank + 1)) / S;
-  for (int idx = t; idx < (r_hi - r_lo) * BN; idx += 256) {
-    const int rr = r_lo + idx / BN, cc = idx % BN;
-    Acc v = Acc(0);
-    for (int q = 0; q < S; ++q) v += *cluster.map_shared_rank(&Ps[rr][cc], q);
-    const int m = m0 + rr, nn = n0 + cc;
-    if (m < a.M && nn < a.N) wg_store(a, m, nn, v);
-  }
-  cluster.sync();
-}
-
-static cudaError_t launch_wgrad(const WgradArgs& a, cudaStream_t st) {
-  const int gx = cdiv(a.N, BN), gy = cdiv(a.M, BM);
-  const int nk = cdiv(a.Kb, BK);
-  int S = 1;
-  const int target = 2 * device_sms();
-  while (S < 8 && gx * gy * S < target && nk / (S * 2) >= 4) S *= 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(gx, gy, S);
-  cfg.blockDim = dim3(256);
-  cfg.stream = st;
-  cudaLaunchAttribute lattr[1];
-  lattr[0].id = cudaLaunchAttributeClusterDimension;
-  lattr[0].val.clusterDim.x = 1; lattr[0].val.clusterDim.y = 1; lattr[0].val.clusterDim.z = S;
-  cfg.attrs = lattr; cfg.numAttrs = 1;
-  if (a.C64) return cudaLaunchKernelEx(&cfg, wgrad_gemm_kernel<double>, a);
-  return cudaLaunchKernelEx(&cfg, wgrad_gemm_kernel<float>, a);
-}
 
 // dst[r, j] += c[r] * src[r, j]
 __global__ void row_axpy_kernel(float* dst, const float* src, const float* c, long long N, int w) {
@@ -293,6 +152,7 @@ GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
   lo.dl[0] = take((size_t)B * smax); lo.dl[1] = take((size_t)B * smax);
   lo.y = take((size_t)B * h->n); lo.v = take((size_t)B * h->n); lo.g = take((size_t)B * h->n);
   lo.a = take((size_t)B * h->n); lo.f = take((size_t)B);
+  lo.wpart = take(wgrad_part_bytes() / sizeof(float));
   lo.tc = off;
   lo.use_tc = gdb_use_tc(h, B);
   if (lo.use_tc) off += picnn_gdb_tc_ws_floats(h, B, nullptr, nullptr);
@@ -381,6 +241,7 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
     WgradArgs w{};   // dWz_L [s_{L-1}, 1] += kappa * sum_b zt_{L-1} o cz_L   (delta_L = 1)
     w.M = sl; w.N = 1; w.Kb = B; w.A = ws + lo.Zt[L - 1]; w.G = gt->cz[L]; w.lda = sl; w.D = nullptr; w.ldd = 1;
     w.C = acc->gr->dWz[L]; w.ldc = 1; w.kappa = kp; w.C64 = acc->w64 ? acc->w64->dWz[L] : nullptr;
+    w.part = ws + lo.wpart;
     GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(L)");
   }
   int cur = 0;
@@ -389,7 +250,7 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
       WgradArgs w{};
       w.M = h->prev(i); w.N = h->hidden[i]; w.Kb = B; w.A = ws + lo.Zt[i - 1]; w.G = gt->cz[i]; w.lda = w.M;
       w.D = dl[cur]; w.ldd = w.N; w.C = acc->gr->dWz[i]; w.ldc = w.N; w.kappa = acc->kappa;
-      w.C64 = acc->w64 ? acc->w64->dWz[i] : nullptr;
+      w.C64 = acc->w64 ? acc->w64->dWz[i] : nullptr; w.part = ws + lo.wpart;
       GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad");
     }
     if (lo.use_tc) {
@@ -420,7 +281,7 @@ int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const 
     WgradArgs w{};
     w.M = n; w.N = h->hidden[l]; w.Kb = B; w.A = av; w.G = gt->cy[l]; w.lda = n;
     w.D = ws + lo.Dacc[l]; w.ldd = w.N; w.C = gr->dWy[l]; w.ldc = w.N; w.kappa = 1.f;
-    w.C64 = w64 ? w64->dWy[l] : nullptr;
+    w.C64 = w64 ? w64->dWy[l] : nullptr; w.part = ws + lo.wpart;
     GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy)");
     GemmArgs a{};   // dcy_l = a o (Delta_l Wy_l^T): the backward GEMM against the Wy rows of Wcat_l
     a.M = B; a.N0 = 0; a.N = n; a.K0 = h->hidden[l]; a.K1 = 0; a.A0 = ws + lo.Dacc[l]; a.lda0 = a.K0;
@@ -431,7 +292,7 @@ int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const 
   // output layer: Delta_L = ksum for every row
   WgradArgs w{};
   w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gt->cy[L]; w.lda = n; w.D = nullptr; w.ldd = 1;
-  w.C = gr->dWy[L]; w.ldc = 1; w.kappa = ksum; w.C64 = w64 ? w64->dWy[L] : nullptr;
+  w.C = gr->dWy[L]; w.ldc = 1; w.kappa = ksum; w.C64 = w64 ? w64->dWy[L] : nullptr; w.part = ws + lo.wpart;
   GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
   rowbcast_fma_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], ksum,
                                                                   N, n);
@@ -529,6 +390,7 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
         w.M = sp; w.N = 1; w.Kb = B; w.A = ws + lo.Sout; w.G = gates->cz[L]; w.lda = sp; w.D = nullptr; w.ldd = 1;
         w.C = gr->dWz[L]; w.ldc = 1; w.kappa = 1.f;
       }
+      w.part = ws + lo.wpart;
       GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad (stored)");
     }
   } else

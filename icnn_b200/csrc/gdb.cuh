@@ -8,6 +8,7 @@ namespace icnn {
 
 struct GdbLayout {
   size_t Z[ICNN_MAX_LAYERS], Zt[ICNN_MAX_LAYERS], Dacc[ICNN_MAX_LAYERS], dl[2], y, v, g, a, f, tc, total;
+  size_t wpart;   // wgrad_part_bytes() (wgrad.cuh): the weight-gradient GEMMs' partial tiles, independent of B
   bool use_tc;
   // stored-pattern mode (single pass): per-iteration stores and the phase-2 scratch
   bool stored;

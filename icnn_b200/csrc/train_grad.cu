@@ -25,6 +25,7 @@
 // (its c sum to zero), so float32 sums would make the result depend on where the chunks are cut.
 #include "gdb.cuh"
 #include "train_rows.cuh"
+#include "wgrad.cuh"
 
 namespace icnn {
 
@@ -54,10 +55,12 @@ static size_t tg_floats(const icnn_picnn* h, long long cap, TgLayout* t) {
   return off;
 }
 
-// rows per chunk: ICNN_TRAIN_CHUNK if set, else what fits ICNN_TRAIN_WS_GB (at least 64, at most R)
+// rows per chunk: ICNN_TRAIN_CHUNK if set, else what fits ICNN_TRAIN_WS_GB (at least 64, at most R); the
+// weight-gradient partials are one fixed region, not per row
 static long long tg_chunk_rows(const icnn_picnn* h, long long R) {
   const long long probe = 1024;
-  return chunk_rows(4.0 * (double)(gdb_layout(h, (int)probe, 0).total + tg_floats(h, probe, nullptr)) / probe, R);
+  const size_t fl = gdb_layout(h, (int)probe, 0).total - wgrad_part_bytes() / sizeof(float) + tg_floats(h, probe, nullptr);
+  return chunk_rows(4.0 * (double)fl / probe, R);
 }
 
 static TgLayout tg_layout(const icnn_picnn* h, int B, long long R) {
