@@ -38,6 +38,7 @@ SYMBOLS = [
     "icnn_conv_solve_batch_fused", "icnn_conv_gd_solve",
     "icnn_conv_train_grad_workspace_bytes", "icnn_conv_train_grad",
     "icnn_conv_gd_backward_workspace_bytes", "icnn_conv_gd_backward",
+    "icnn_td_grad_workspace_bytes", "icnn_td_grad",
 ]
 
 _fpp = C.POINTER(C.c_void_p)
@@ -163,6 +164,11 @@ def _load():
     lib.icnn_conv_gd_backward.argtypes = [C.c_void_p, C.POINTER(Gates), C.c_void_p, C.c_void_p, C.c_float, C.c_int32,
                                           C.c_float, C.c_float, C.c_void_p, C.POINTER(ConvTrainGrads), C.c_void_p,
                                           C.c_void_p]
+    lib.icnn_td_grad_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    lib.icnn_td_grad_workspace_bytes.restype = C.c_size_t
+    lib.icnn_td_grad.argtypes = [C.c_void_p, C.POINTER(Gates), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.POINTER(TrainGrads), C.c_void_p,
+                                 C.c_void_p]
     for name in SYMBOLS:
         getattr(lib, name)  # AttributeError if the .so does not export it
     if lib.icnn_abi_version() != ABI_VERSION:

@@ -63,19 +63,26 @@ def _check_conv_x(fg, x, who):
     return True
 
 
-def _prepare(fg, offsets):
-    """Output buffers, the C structs and the workspace of one icnn_train_grad call for the CSR ``offsets``."""
+def _grad_buffers(fg):
+    """Output buffers of the icnn_train_grads layout for ``fg``'s batch, the host pointer arrays and the C struct."""
     net, dev, B = fg.net, fg.net.device, fg.B
     n, L, hid = net.n, net.L, net.hidden
     width = lambda l: hid[l] if l < L else 1          # noqa: E731
     prev = lambda l: hid[l - 1]                        # noqa: E731
-    R = int(offsets[-1])
     z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
     grads = dict(Wy=[z(n, width(l)) for l in range(L + 1)], Wz=[None] + [z(prev(l), width(l)) for l in range(1, L + 1)],
                  dcy=[z(B, n) for _ in range(L + 1)], dcz=[None] + [z(B, prev(l)) for l in range(1, L + 1)],
                  dd=[z(B, width(l)) for l in range(L + 1)])
     arrs = [_capi.ptr_array(grads[k]) for k in ("Wy", "Wz", "dcy", "dcz", "dd")]
     gr = _capi.TrainGrads(*[C.cast(a, _capi._fpp) for a in arrs])
+    return grads, arrs, gr
+
+
+def _prepare(fg, offsets):
+    """Output buffers, the C structs and the workspace of one icnn_train_grad call for the CSR ``offsets``."""
+    net, dev, B = fg.net, fg.net.device, fg.B
+    R = int(offsets[-1])
+    grads, arrs, gr = _grad_buffers(fg)
     off = (C.c_int64 * (B + 1))(*[int(o) for o in offsets])
     ws = torch.empty(max(_capi.lib.icnn_train_grad_workspace_bytes(net._h, B, R), 4), dtype=torch.uint8, device=dev)
     return dict(grads=grads, arrs=arrs, gr=gr, off=off, ws=ws)

@@ -65,10 +65,11 @@ __global__ void axpy_kernel(float* dst, const float* src, float kappa, long long
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i < N) dst[i] = fmaf(kappa, src[i], dst[i]);
 }
-// dst[b, j] += kappa * src[b, j] * w[j]
-__global__ void rowbcast_fma_kernel(float* dst, const float* src, const float* w, float kappa, long long N, int width) {
+// dst[b, j] += kappa * rs[b] * src[b, j] * w[j]   (rs == nullptr: 1)
+__global__ void rowbcast_fma_kernel(float* dst, const float* src, const float* w, const float* rs, float kappa,
+                                    long long N, int width) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < N) dst[i] = fmaf(kappa * src[i], w[i % width], dst[i]);
+  if (i < N) dst[i] = fmaf((rs ? kappa * rs[i / width] : kappa) * src[i], w[i % width], dst[i]);
 }
 // a = scale * (y - trueY)      (d/dy_N of scale/2 * sum (y_N - trueY)^2)
 __global__ void mse_grad_kernel(float* a, const float* y, const float* trueY, float scale, long long N) {
@@ -182,34 +183,52 @@ GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
     if (_le != cudaSuccess) { set_error("%s launch: %s", what, cudaGetErrorString(_le)); return ICNN_E_CUDA; } \
   } while (0)
 
+// The buffers of the tensor-core GEMMs of one iteration, with the optional epilogue accumulations / stores.
+static GdbTcBufs gdb_tc_bufs(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo,
+                             const GdbAcc* acc, int store_it, float store_kappa) {
+  const int B = gt->B, L = h->L;
+  GdbTcBufs tb{};
+  tb.y = ws + lo.y; tb.g = ws + lo.g; tb.dp[0] = ws + lo.dl[0]; tb.dp[1] = ws + lo.dl[1];
+  const bool primal_op = acc && acc->dL;   // td_grad: the accumulations take Z_l where the tangent pass takes Zt_l
+  for (int i = 0; i < L; ++i) {
+    tb.Z[i] = ws + lo.Z[i]; tb.Zt[i] = ws + (primal_op ? lo.Z[i] : lo.Zt[i]); tb.Dacc[i] = ws + lo.Dacc[i];
+  }
+  if (acc) {
+    tb.want_plain = true; tb.acc_delta = true; tb.kappa = acc->kappa;
+    for (int i = 1; i < L; ++i) tb.dcz[i] = acc->gr->dcz[i];
+  }
+  if (store_it >= 0) {
+    tb.want_plain = true; tb.acc_delta = true; tb.kappa = store_kappa;
+    for (int i = 0; i < L; ++i) {
+      const size_t r = (size_t)store_it * B;
+      tb.Z[i] = ws + lo.Zs[i] + r * h->hidden[i];
+      tb.dstore[i] = ws + lo.Ds[i] + r * h->hidden[i];
+      if (i > 0) tb.astore[i] = ws + lo.As[i] + r * h->prev(i);
+    }
+  }
+  picnn_gdb_tc_ws_floats(h, B, &tb, ws + lo.tc);
+  return tb;
+}
+
 // One GD iteration's primal forward + backward.  acc != nullptr: also the tangent forward and the
 // gradient accumulations (pass 2 of the two-pass mode).  store_it >= 0 (stored-pattern mode, tensor-core
 // path only): the primal pass writes Z_l, delta_l and delta_l Wz_l^T of this iteration into the stores
 // and accumulates Delta_l += kappa delta_l.  (GdbAcc: gdb.cuh)
 int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo,
                   const GdbAcc* acc, int store_it, float store_kappa, cudaStream_t st) {
+  const int rc = gdb_forward(h, gt, ws, lo, acc, store_it, store_kappa, st);
+  return rc ? rc : gdb_backward(h, gt, ws, lo, acc, store_it, store_kappa, st);
+}
+
+int gdb_forward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo, const GdbAcc* acc,
+                int store_it, float store_kappa, cudaStream_t st) {
   const int B = gt->B, n = h->n, L = h->L;
   float* y = ws + lo.y; float* g = ws + lo.g; float* f = ws + lo.f; float* av = ws + lo.a;
-  float* dl[2] = {ws + lo.dl[0], ws + lo.dl[1]};
+  const bool tangent = acc && !acc->dL;
   GdbTcBufs tb{};
   if (lo.use_tc) {
-    tb.y = y; tb.g = g; tb.dp[0] = dl[0]; tb.dp[1] = dl[1];
-    for (int i = 0; i < L; ++i) { tb.Z[i] = ws + lo.Z[i]; tb.Zt[i] = ws + lo.Zt[i]; tb.Dacc[i] = ws + lo.Dacc[i]; }
-    if (acc) {
-      tb.want_plain = true; tb.acc_delta = true; tb.kappa = acc->kappa;
-      for (int i = 1; i < L; ++i) tb.dcz[i] = acc->gr->dcz[i];
-    }
-    if (store_it >= 0) {
-      tb.want_plain = true; tb.acc_delta = true; tb.kappa = store_kappa;
-      for (int i = 0; i < L; ++i) {
-        const size_t r = (size_t)store_it * B;
-        tb.Z[i] = ws + lo.Zs[i] + r * h->hidden[i];
-        tb.dstore[i] = ws + lo.Ds[i] + r * h->hidden[i];
-        if (i > 0) tb.astore[i] = ws + lo.As[i] + r * h->prev(i);
-      }
-    }
-    picnn_gdb_tc_ws_floats(h, B, &tb, ws + lo.tc);
-    int rc = picnn_gdb_tc_forward(h, gt, tb, acc != nullptr, st);
+    tb = gdb_tc_bufs(h, gt, ws, lo, acc, store_it, store_kappa);
+    int rc = picnn_gdb_tc_forward(h, gt, tb, tangent, st);
     if (rc) return rc;
   }
   for (int i = 0; i < L && !lo.use_tc; ++i) {
@@ -219,7 +238,7 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
     a.A1 = y; a.G1 = gt->cy[i]; a.lda1 = n; a.a1_scale = 1.f; a.a1_shift = 0.f;
     a.W = h->Wcat[i]; a.ldw = a.N; a.D = gt->d[i]; a.Z = ws + lo.Z[i]; a.alpha = h->alpha;
     GDB_LAUNCH(launch_gemm<0>(a, st), "gd_backward forward");
-    if (acc) {   // tangent layer: same product on (zt_{i-1}, a), pattern of Z_i, no bias
+    if (tangent) {   // tangent layer: same product on (zt_{i-1}, a), pattern of Z_i, no bias
       a.A0 = i ? ws + lo.Zt[i - 1] : nullptr; a.A1 = av; a.D = nullptr;
       a.Zmask = ws + lo.Z[i]; a.Z = ws + lo.Zt[i];
       GDB_LAUNCH(launch_gemm<2>(a, st), "gd_backward tangent");
@@ -227,19 +246,32 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
   }
   if (acc && acc->c)   // train_grad: the backward accumulates with c o Z_l + Zt_l in place of the tangent
     for (int i = 0; i < L; ++i) launch_row_axpy(ws + lo.Zt[i], ws + lo.Z[i], acc->c, B, h->hidden[i], st);
-  const int sl = h->hidden[L - 1];
-  const long long NL = (long long)B * sl;
-  float* dlast = store_it >= 0 ? tb.dstore[L - 1] : dl[0];     // plain delta_{L-1}
+  float* dlast = store_it >= 0 ? tb.dstore[L - 1] : ws + lo.dl[0];     // plain delta_{L-1}
   out_layer_launch(h, gt, lo.use_tc ? tb.Z[L - 1] : ws + lo.Z[L - 1], y, f, dlast, lo.use_tc ? tb.dh[0] : nullptr,
                    lo.use_tc ? tb.dl[0] : nullptr, g, n, nullptr, nullptr, 0, nullptr, st);
-  if (store_it >= 0) axpy_kernel<<<(unsigned)((NL + 255) / 256), 256, 0, st>>>(ws + lo.Dacc[L - 1], dlast, store_kappa, NL);
+  return ICNN_OK;
+}
+
+int gdb_backward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo, const GdbAcc* acc,
+                 int store_it, float store_kappa, cudaStream_t st) {
+  const int B = gt->B, L = h->L;
+  float* g = ws + lo.g;
+  float* dl[2] = {ws + lo.dl[0], ws + lo.dl[1]};
+  GdbTcBufs tb{};
+  if (lo.use_tc) tb = gdb_tc_bufs(h, gt, ws, lo, acc, store_it, store_kappa);
+  // the backward's accumulation operand of layer i: the tangent Zt_i, or with GdbAcc::dL the primal Z_i
+  auto zt = [&](int i) { return ws + (acc && acc->dL ? lo.Z[i] : lo.Zt[i]); };
+  const int sl = h->hidden[L - 1];
+  const long long NL = (long long)B * sl;
+  if (store_it >= 0) axpy_kernel<<<(unsigned)((NL + 255) / 256), 256, 0, st>>>(ws + lo.Dacc[L - 1], tb.dstore[L - 1],
+                                                                                store_kappa, NL);
   if (acc) {
     const float kp = acc->kappa;
     axpy_kernel<<<(unsigned)((NL + 255) / 256), 256, 0, st>>>(ws + lo.Dacc[L - 1], dl[0], kp, NL);
-    rowbcast_fma_kernel<<<(unsigned)((NL + 255) / 256), 256, 0, st>>>(acc->gr->dcz[L], ws + lo.Zt[L - 1],
-                                                                      h->Wcat[L], kp, NL, sl);
-    WgradArgs w{};   // dWz_L [s_{L-1}, 1] += kappa * sum_b zt_{L-1} o cz_L   (delta_L = 1)
-    w.M = sl; w.N = 1; w.Kb = B; w.A = ws + lo.Zt[L - 1]; w.G = gt->cz[L]; w.lda = sl; w.D = nullptr; w.ldd = 1;
+    rowbcast_fma_kernel<<<(unsigned)((NL + 255) / 256), 256, 0, st>>>(acc->gr->dcz[L], zt(L - 1), h->Wcat[L], acc->dL,
+                                                                      kp, NL, sl);
+    WgradArgs w{};   // dWz_L [s_{L-1}, 1] += kappa * sum_b zt_{L-1} o cz_L delta_L   (delta_L = 1, or dL[b])
+    w.M = sl; w.N = 1; w.Kb = B; w.A = zt(L - 1); w.G = gt->cz[L]; w.lda = sl; w.D = acc->dL; w.ldd = 1;
     w.C = acc->gr->dWz[L]; w.ldc = 1; w.kappa = kp; w.C64 = acc->w64 ? acc->w64->dWz[L] : nullptr;
     w.part = ws + lo.wpart;
     GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(L)");
@@ -248,7 +280,7 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
   for (int i = L - 1; i >= 0; --i) {
     if (acc && i > 0) {   // dWz_i += kappa (zt_{i-1} o cz_i)^T delta_i
       WgradArgs w{};
-      w.M = h->prev(i); w.N = h->hidden[i]; w.Kb = B; w.A = ws + lo.Zt[i - 1]; w.G = gt->cz[i]; w.lda = w.M;
+      w.M = h->prev(i); w.N = h->hidden[i]; w.Kb = B; w.A = zt(i - 1); w.G = gt->cz[i]; w.lda = w.M;
       w.D = dl[cur]; w.ldd = w.N; w.C = acc->gr->dWz[i]; w.ldc = w.N; w.kappa = acc->kappa;
       w.C64 = acc->w64 ? acc->w64->dWz[i] : nullptr; w.part = ws + lo.wpart;
       GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad");
@@ -260,12 +292,12 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
       continue;
     }
     GemmArgs a{};
-    a.M = B; a.N0 = h->prev(i); a.N = a.N0 + n; a.K0 = h->hidden[i]; a.K1 = 0;
+    a.M = B; a.N0 = h->prev(i); a.N = a.N0 + h->n; a.K0 = h->hidden[i]; a.K1 = 0;
     a.A0 = dl[cur]; a.lda0 = a.K0; a.W = h->Wcat[i]; a.ldw = a.K0; a.alpha = h->alpha;
     a.Zprev = i ? ws + lo.Z[i - 1] : nullptr; a.Cz = i ? gt->cz[i] : nullptr; a.dprev = dl[cur ^ 1];
-    a.Cy = gt->cy[i]; a.g = g; a.g_row_stride = n; a.n = n; a.g_scale = 1.f;
+    a.Cy = gt->cy[i]; a.g = g; a.g_row_stride = h->n; a.n = h->n; a.g_scale = 1.f;
     if (acc && i > 0) {
-      a.dCz = acc->gr->dcz[i]; a.Ztprev = ws + lo.Zt[i - 1]; a.Dacc = ws + lo.Dacc[i - 1]; a.kappa = acc->kappa;
+      a.dCz = acc->gr->dcz[i]; a.Ztprev = zt(i - 1); a.Dacc = ws + lo.Dacc[i - 1]; a.kappa = acc->kappa;
     }
     GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward backward");
     cur ^= 1;
@@ -274,7 +306,7 @@ int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gd
 }
 
 int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo, const float* av,
-                    const icnn_gd_grads* gr, float ksum, const GdbW64* w64, cudaStream_t st) {
+                    const icnn_gd_grads* gr, float ksum, const GdbW64* w64, const float* dL, cudaStream_t st) {
   const int B = gt->B, n = h->n, L = h->L;
   const long long N = (long long)B * n;
   for (int l = 0; l < L; ++l) {
@@ -289,13 +321,13 @@ int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const 
     a.Cy = av; a.g = gr->dcy[l]; a.g_row_stride = n; a.n = n; a.g_scale = 1.f;
     GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward dcy");
   }
-  // output layer: Delta_L = ksum for every row
+  // output layer: Delta_L = ksum for every row (times dL[row] when given)
   WgradArgs w{};
-  w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gt->cy[L]; w.lda = n; w.D = nullptr; w.ldd = 1;
+  w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gt->cy[L]; w.lda = n; w.D = dL; w.ldd = 1;
   w.C = gr->dWy[L]; w.ldc = 1; w.kappa = ksum; w.C64 = w64 ? w64->dWy[L] : nullptr; w.part = ws + lo.wpart;
   GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
-  rowbcast_fma_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], ksum,
-                                                                  N, n);
+  rowbcast_fma_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], dL,
+                                                                  ksum, N, n);
   return ICNN_OK;
 }
 
@@ -415,7 +447,7 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
   }
 
   if (nIter > 0) {
-    int rc = gdb_ygate_stage(h, gates, ws, lo, av, gr, (float)ksum, nullptr, st);
+    int rc = gdb_ygate_stage(h, gates, ws, lo, av, gr, (float)ksum, nullptr, nullptr, st);
     if (rc) return rc;
   }
   ICNN_CUDA_CHECK(cudaGetLastError());

@@ -195,7 +195,7 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
     int rc = gdb_iteration(h, &gt, ws, lo, &acc, -1, 0.f, st);
     if (rc) return rc;
     launch_row_axpy(ws + lo.a, ws + lo.y, c + r0, rows, n, st);   // yhat = c y + v
-    rc = gdb_ygate_stage(h, &gt, ws, lo, ws + lo.a, &rg, 1.f, &w64, st);
+    rc = gdb_ygate_stage(h, &gt, ws, lo, ws + lo.a, &rg, 1.f, &w64, nullptr, st);
     if (rc) return rc;
 
     // per-row gate adjoints -> per-sample outputs; dd_l = sum_r c_r delta_l (delta_L = 1)

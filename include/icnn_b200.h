@@ -257,6 +257,25 @@ size_t icnn_train_grad_workspace_bytes(const icnn_picnn_t* h, int32_t B, int64_t
 int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, const int64_t* row_offsets, const float* Y,
                     const float* V, const float* c, const icnn_train_grads* grads, void* workspace, void* stream);
 
+/* ---- RL TD training gradient (the training step after Agent.adam) ------------------------------------- */
+/* replaces: optim_q.compute_gradients(loss_q) (RL/src/icnn.py:107-108) of the '--icnn_opt adam' agent
+ * (RL/src/icnn.py:55-93, Agent.train :304-323) for the y-path of the online network 'q':
+ *   q_entr = -(negQ(obs, act) - H(act)),  q_target_entr = -(negq_target - H(act2))
+ *   y = term ? rew : rew + discount q_target_entr,  y = min(q_entr + 1, max(q_entr - 1, y))  (stop_gradient)
+ *   td = q_entr - y,  loss = mean(td^2)   (ms_td_error; the L2 term of loss_q is the caller's)
+ * with H(a) = -sum_j p log p + (1 - p) log(1 - p), p = clip((a + 1) / 2, 1e-4, 1 - 1e-4) (:455-458).  gates are
+ * those of obs bound WITHOUT the affine wrapper (ICNN_E_UNSUPPORTED otherwise); act, act2 [B, n], negq_target
+ * (K1's f of the target network at act2), rew [B] device f32, term [B] device uint8 (0 / 1).  Outputs: td [B] f32,
+ * loss [1] f64 (fixed-order sum), and d loss / d (y-path weights and gates) in the icnn_train_grads layout, all
+ * overwritten: dWy / dWz summed over the batch, dcy / dcz / dd per sample.  The result equals icnn_train_grad at
+ * Y = act, V = 0, c = -2 td / B with one row per sample; this entry runs one forward and no tangent network.
+ * B <= 65536 (ICNN_E_INVALID above); workspace = icnn_td_grad_workspace_bytes(h, B) device bytes (0 for an invalid
+ * B).  Deterministic: two calls give the same bits. */
+size_t icnn_td_grad_workspace_bytes(const icnn_picnn_t* h, int32_t B);
+int icnn_td_grad(const icnn_picnn_t* h, const icnn_gates* gates, const float* act, const float* negq_target,
+                 const float* act2, const float* rew, const uint8_t* term, float discount, float* td, double* loss,
+                 const icnn_train_grads* grads, void* workspace, void* stream);
+
 /* ---- RL Adam argmin (SURVEY.md section 8f, row 3) -------------------------------------------------- */
 /* replaces: Agent.adam (RL/src/icnn.py:160-215) applied to [negQ - entropy(act), d/dact]
  * (RL/src/icnn.py:60-63,127-131,455-458): batched Adam on the actions with best-so-far tracking and
