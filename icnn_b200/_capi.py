@@ -10,6 +10,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libicnn_b200.so")
 
@@ -191,3 +193,13 @@ def ptr_array(tensors):
     for i, t in enumerate(tensors):
         arr[i] = None if t is None else t.data_ptr()
     return arr
+
+
+def workspace(nbytes, device):
+    """Device workspace of ``nbytes`` bytes (at least 4: ``torch.empty(0)`` would hand the library a null pointer)."""
+    return torch.empty(max(nbytes, 4), dtype=torch.uint8, device=device)
+
+
+def stream():
+    """The current CUDA stream as the library's ``stream`` argument."""
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)

@@ -37,62 +37,27 @@ import torch
 
 from . import _capi
 from .argmin_grad import LOSS, argmin_grad
-from .gd_grad import _f32, _xpath_backward
-from .conv_picnn import BoundConvPICNN, _gate_vjp, _to_host, _train_grad_buffers, _ypath_grads, conv_trainable
+from .conv_picnn import _gate_vjp, _train_grad_buffers, _ypath_grads, conv_trainable
+from .gd_grad import _check_fg, _f32, _grad_buffers, _host, _xpath_backward
 from .picnn import BoundPICNN
 
 # parameter names of the returned dictionary with x given (the PICNN attribute names)
 PARAMS = ("Wy", "Wz", "Wu", "bu", "Wzu", "bzu", "Wyu", "byu", "Wzx", "bzx")
 
 
-def _check_fg(fg, who):
-    if isinstance(fg, BoundConvPICNN):
-        return
-    if not isinstance(fg, BoundPICNN):
-        raise TypeError("%s needs a BoundPICNN (PICNN.bind(x)) or a BoundConvPICNN (ConvPICNN.bind(x))" % who)
-    if fg.affine:
-        raise ValueError("%s: the affine RL wrapper has no bundle training step (RL/src/icnn.py:84)" % who)
-
-
-def _check_conv_x(fg, x, who):
-    """True for a conv fg (whose x-path uses the minibatch it was bound to: ``x`` is refused)."""
-    if not isinstance(fg, BoundConvPICNN):
-        return False
-    if x is not None:
-        raise ValueError("%s: a BoundConvPICNN uses the minibatch it was bound to; do not pass x" % who)
-    return True
-
-
-def _grad_buffers(fg):
-    """Output buffers of the icnn_train_grads layout for ``fg``'s batch, the host pointer arrays and the C struct."""
-    net, dev, B = fg.net, fg.net.device, fg.B
-    n, L, hid = net.n, net.L, net.hidden
-    width = lambda l: hid[l] if l < L else 1          # noqa: E731
-    prev = lambda l: hid[l - 1]                        # noqa: E731
-    z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-    grads = dict(Wy=[z(n, width(l)) for l in range(L + 1)], Wz=[None] + [z(prev(l), width(l)) for l in range(1, L + 1)],
-                 dcy=[z(B, n) for _ in range(L + 1)], dcz=[None] + [z(B, prev(l)) for l in range(1, L + 1)],
-                 dd=[z(B, width(l)) for l in range(L + 1)])
-    arrs = [_capi.ptr_array(grads[k]) for k in ("Wy", "Wz", "dcy", "dcz", "dd")]
-    gr = _capi.TrainGrads(*[C.cast(a, _capi._fpp) for a in arrs])
-    return grads, arrs, gr
-
-
 def _prepare(fg, offsets):
     """Output buffers, the C structs and the workspace of one icnn_train_grad call for the CSR ``offsets``."""
     net, dev, B = fg.net, fg.net.device, fg.B
-    R = int(offsets[-1])
-    grads, arrs, gr = _grad_buffers(fg)
+    grads, arrs, gr = _grad_buffers(fg, dd=True)
     off = (C.c_int64 * (B + 1))(*[int(o) for o in offsets])
-    ws = torch.empty(max(_capi.lib.icnn_train_grad_workspace_bytes(net._h, B, R), 4), dtype=torch.uint8, device=dev)
+    ws = _capi.workspace(_capi.lib.icnn_train_grad_workspace_bytes(net._h, B, int(offsets[-1])), dev)
     return dict(grads=grads, arrs=arrs, gr=gr, off=off, ws=ws)
 
 
 def _launch(fg, prep, Y, V, c):
     """icnn_train_grad on the current stream (asynchronous; ``prep`` and the inputs must outlive the work)."""
-    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     _capi.check(_capi.lib.icnn_train_grad(fg.net._h, C.byref(fg.c_gates), prep["off"], Y.data_ptr(), V.data_ptr(),
-                                          c.data_ptr(), C.byref(prep["gr"]), prep["ws"].data_ptr(), stream))
+                                          c.data_ptr(), C.byref(prep["gr"]), prep["ws"].data_ptr(), _capi.stream()))
 
 
 def _run(fg, Y, V, c, offsets, x, return_device):
@@ -102,10 +67,7 @@ def _run(fg, Y, V, c, offsets, x, return_device):
     if x is not None:
         grads.update(_xpath_backward(fg.net, _f32(x, fg.net.device), grads["dcy"], grads["dcz"], grads["dd"]))
     torch.cuda.current_stream().synchronize()      # ws / arrs / the inputs stay alive until the work is done
-    if return_device:
-        return grads
-    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
-    return {k: [host(t) for t in v] for k, v in grads.items()}
+    return grads if return_device else _host(grads)
 
 
 def _conv_launch(fg, Y, V, c, offsets):
@@ -115,11 +77,9 @@ def _conv_launch(fg, Y, V, c, offsets):
     R = int(offsets[-1])
     o, gr, arrs = _train_grad_buffers(fg)
     off = (C.c_int64 * (B + 1))(*[int(o_) for o_ in offsets])
-    ws = torch.empty(max(_capi.lib.icnn_conv_train_grad_workspace_bytes(net._h, B, R), 4), dtype=torch.uint8,
-                     device=dev)
-    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    ws = _capi.workspace(_capi.lib.icnn_conv_train_grad_workspace_bytes(net._h, B, R), dev)
     _capi.check(_capi.lib.icnn_conv_train_grad(net._h, C.byref(fg.c_gates), off, Y.data_ptr(), V.data_ptr(),
-                                               c.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
+                                               c.data_ptr(), C.byref(gr), ws.data_ptr(), _capi.stream()))
     return dict(o, keep=(arrs, gr, off, ws))
 
 
@@ -133,7 +93,7 @@ def _conv_run(fg, Y, V, c, offsets, return_device):
     grads = {k: grads[k] for k in conv_trainable(net)}
     grads.update(dcy=o["dcy"], dcz=o["dcz"], dd=o["dd"])
     torch.cuda.current_stream().synchronize()      # ws / arrs / the inputs stay alive until the work is done
-    return grads if return_device else _to_host(grads)
+    return grads if return_device else _host(grads)
 
 
 def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):
@@ -152,8 +112,7 @@ def train_grad(fg: BoundPICNN, Y, V, c, counts, x=None, return_device=False):
     (the x-path from the minibatch ``fg`` was bound to; ``x`` is refused), plus 'dcy' (per conv layer), 'dcz' and
     'dd' (per layer, [B, flat gate]); numpy arrays, or with ``return_device=True`` torch tensors on the net's device
     (for ``net.vars[k].grad = g``)."""
-    _check_fg(fg, "train_grad")
-    conv = _check_conv_x(fg, x, "train_grad")
+    conv = _check_fg(fg, "train_grad", x)
     net, dev, B = fg.net, fg.net.device, fg.B
     counts = np.asarray(counts.cpu() if isinstance(counts, torch.Tensor) else counts, dtype=np.int64).reshape(-1)
     if counts.shape != (B,) or (counts < 0).any():
@@ -175,8 +134,7 @@ def bundle_grad(fg: BoundPICNN, state, trueY, loss="xent", x=None, return_device
     ``train_grad``.  ``state`` is the ``BundleState`` of ``solveBatch(fg, ..., return_state=True)`` (solved with
     ``keep_xs=True``, the default); ``trueY`` [B, n] the labels; ``loss`` 'xent' or 'mse'.  Same return layout as
     ``train_grad``."""
-    _check_fg(fg, "bundle_grad")
-    conv = _check_conv_x(fg, x, "bundle_grad")
+    conv = _check_fg(fg, "bundle_grad", x)
     if loss not in LOSS:
         raise ValueError("loss must be 'mse' or 'xent'")
     if state.B != fg.B or state.n != fg.net.n:

@@ -372,8 +372,3 @@ def _gate_vjp(fg, names, dcy, dcz, dd):
         s = s + sum((gd[i].reshape(B, -1) * dd[i]).sum() for i in range(NL))
         xg = torch.autograd.grad(s, [P[k] for k in names])
     return dict(zip(names, (g.detach() for g in xg)))
-
-
-def _to_host(grads):
-    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
-    return {k: [host(t) for t in v] if isinstance(v, list) else host(v) for k, v in grads.items()}

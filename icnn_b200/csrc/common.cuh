@@ -23,7 +23,17 @@ void set_error(const char* fmt, ...);
     }                                                                                \
   } while (0)
 
-#define ICNN_REQUIRE(cond, msg)                                        \
+// a failed launch (or any error a launch stage leaves): "<entry> <stage>: <cuda error>"
+#define ICNN_LAUNCH_CHECK(expr, what)                                                \
+  do {                                                                               \
+    cudaError_t _le = (expr);                                                        \
+    if (_le != cudaSuccess) {                                                        \
+      icnn::set_error("%s: %s", what, cudaGetErrorString(_le));                      \
+      return ICNN_E_CUDA;                                                            \
+    }                                                                                \
+  } while (0)
+
+#define ICNN_REQUIRE(cond, msg)                                     \
   do {                                                                 \
     if (!(cond)) {                                                     \
       icnn::set_error("%s:%d: invalid argument: %s", __FILE__, __LINE__, msg); \

@@ -219,12 +219,6 @@ static CtgLayout ctg_layout(const icnn_conv_picnn* h, int B, long long R) {
   return t;
 }
 
-#define CTG_LAUNCH(what)                                                                                \
-  do {                                                                                                  \
-    cudaError_t _le = cudaGetLastError();                                                               \
-    if (_le != cudaSuccess) { set_error("conv_train_grad %s: %s", what, cudaGetErrorString(_le)); return ICNN_E_CUDA; } \
-  } while (0)
-
 // every per-layer buffer of icnn_conv_train_grads the layers use is given
 static int ctg_check_buffers(const icnn_conv_picnn* h, const icnn_conv_train_grads* gr) {
   const int Lc = h->Lc, NL = h->Lc + h->Ld;
@@ -294,11 +288,8 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
   int rc = conv_check_gates(h, gates);
   if (rc) return rc;
   const int B = gates->B, Lc = h->Lc, Ld = h->Ld, NL = Lc + Ld, n = h->H * h->W;
-  ICNN_REQUIRE(row_offsets[0] == 0, "row_offsets[0] != 0");
-  for (int u = 0; u < B; ++u) ICNN_REQUIRE(row_offsets[u + 1] >= row_offsets[u], "row_offsets decreasing");
-  const long long R = row_offsets[B];
-  ICNN_REQUIRE(R <= INT32_MAX, "more than 2^31 - 1 rows");
-  ICNN_REQUIRE(R == 0 || (Y && V && c), "null row input");
+  const long long R = check_row_offsets(row_offsets, B, Y && V && c);
+  if (R < 0) return (int)R;
   if ((rc = ctg_check_buffers(h, gr))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
@@ -354,11 +345,8 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
       gt.B = rows;
 
       // ---- per-row gates ----
-      row_sample_kernel<<<cdiv(rows, 256), 256, 0, st>>>(row_u, off_d, u0, u1, r0, rows);
-      auto gather = [&](float* dst, const float* src, long long wdt) {
-        const long long N = (long long)rows * wdt;
-        gather_rows_kernel<<<nb(N), 256, 0, st>>>(dst, src, row_u, N, (int)wdt);
-      };
+      launch_row_sample(row_u, off_d, u0, u1, r0, rows, st);
+      auto gather = [&](float* dst, const float* src, long long wdt) { launch_gather_rows(dst, src, row_u, rows, wdt, st); };
       for (int l = 0; l < Lc; ++l) {
         const ConvGeom& g = h->g[l];
         gather(cy[l], gates->cy[l], (long long)g.Hi * g.Wi);
@@ -369,7 +357,7 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
         gather(cz[Lc + j], gates->cz[Lc + j], h->in_w(j));
         gather(dd[Lc + j], gates->d[Lc + j], h->fcs[j]);
       }
-      CTG_LAUNCH("gather");
+      ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad gather");
 
       // ---- primal: f, df/dy and the un-gated conv adjoints e_l ----
       if ((rc = conv_fg(h, &gt, Yc, fbuf, gbuf, n, nullptr, nullptr, 0, fl + t.cws, nullptr, st, e))) return rc;
@@ -407,7 +395,7 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
         launch_row_axpy(rt[l], l ? w.r[l] : Yc, cc, rows, G.Hi * G.Wi, st);
       }
       for (int j = 0; j + 1 < Ld; ++j) launch_row_axpy(zt[Lc + j], w.fZ[j], cc, rows, h->fcs[j], st);
-      CTG_LAUNCH("tangent");
+      ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad tangent");
 
       // ---- weight gradients (float64 over the rows) ----
       for (int l = 0; l < Lc; ++l) {
@@ -419,14 +407,14 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
         a.D = w.dh[l]; a.Dlo = w.dl[l]; a.ldd = ld4(G.C); a.C64 = acc64 + t.aw[l]; a.ldc = G.C; a.kappa = 1.f;
         a.part = part64;
         launch_wgrad(a, st);
-        CTG_LAUNCH("weight gradient");
+        ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad weight gradient");
         if (l + 1 < Lc) {   // acc += the y_red partials in rank order: the reduce of an M = 1 weight gradient
           WgradArgs r{};
           r.M = 1; r.N = G.k * G.k + 1; r.C64 = acc64 + t.ared[l]; r.ldc = r.N; r.kappa = 1.f; r.part = part64;
           const int P = yred_parts(M);
           yred_grad_kernel<<<dim3(r.N, P), 256, 0, st>>>(rt[l], w.rho[l + 1], cc, G, M, part64);
           wgrad_reduce_kernel<double><<<nb(r.N), 256, 0, st>>>(r, P);
-          CTG_LAUNCH("y_red gradient");
+          ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad y_red gradient");
         }
       }
       for (int j = 0; j < Ld; ++j) {
@@ -436,13 +424,12 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
         if (j + 1 < Ld) { a.D = w.fdh[j]; a.Dlo = w.fdl[j]; a.ldd = ld4(h->fcs[j]); }
         a.C64 = acc64 + t.aw[i]; a.ldc = a.N; a.kappa = 1.f; a.part = part64;
         launch_wgrad(a, st);
-        CTG_LAUNCH("weight gradient");
+        ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad weight gradient");
       }
 
       // ---- per-sample gate adjoints ----
-      const long long NS = (long long)(u1 - u0);
       auto seg = [&](float* out, SegView a, SegView ev, const float* scale, long long wdt) {
-        segsum_prod_kernel<<<nb(NS * wdt), 256, 0, st>>>(out, a, ev, scale, (int)wdt, off_d, u0, u1, r0, r1);
+        launch_segsum_prod(out, a, ev, scale, wdt, off_d, u0, u1, r0, r1, st);
       };
       const SegView one{nullptr, nullptr, 0, 1, 0, 0};
       for (int l = 0; l < Lc; ++l) {
@@ -465,7 +452,7 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
           seg(gr->dd[i], one, one, c, 1);
         }
       }
-      CTG_LAUNCH("segmented sum");
+      ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad segmented sum");
       r0 = r1;
     }
   }
@@ -484,7 +471,7 @@ extern "C" int icnn_conv_train_grad(const icnn_conv_picnn_t* h, const icnn_gates
     const long long N = (long long)h->in_w(j) * h->fcs[j];
     round_to_float_kernel<<<nb(N), 256, 0, st>>>(gr->dWz[Lc + j], acc64 + t.aw[Lc + j], N);
   }
-  CTG_LAUNCH("round");
+  ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad round");
   return ICNN_OK;
 }
 
@@ -534,7 +521,7 @@ extern "C" int icnn_conv_gd_backward(const icnn_conv_picnn_t* h, const icnn_gate
     // (pageable source: the call returns once kappa has been staged)
     ICNN_CUDA_CHECK(cudaMemcpyAsync(kap, kappa.data(), sizeof(float) * nIter, cudaMemcpyHostToDevice, st));
     gd_seed_kernel<<<nb(RN), 256, 0, st>>>(V, c, yN, trueY, kap, loss_scale, nIter, n, RN);
-    CTG_LAUNCH("GD row seeds");
+    ICNN_LAUNCH_CHECK(cudaGetLastError(), "conv_train_grad GD row seeds");
   }
 
   // ---- the training gradient of those rows: sample u owns rows [u nIter, (u + 1) nIter) ----

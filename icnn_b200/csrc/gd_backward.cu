@@ -38,8 +38,6 @@
 namespace icnn {
 
 size_t picnn_simt_ws_floats(const icnn_picnn* h, int B, size_t* zoff, size_t* doff);
-size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* base);
-void picnn_gdb_tc_gate_a(const icnn_picnn* h, const icnn_gates* gt, const float* a, const GdbTcBufs& b, cudaStream_t st);
 int picnn_gdb_tc_forward(const icnn_picnn* h, const icnn_gates* gt, const GdbTcBufs& b, bool tangent, cudaStream_t st);
 int picnn_gdb_tc_backward_layer(const icnn_picnn* h, const icnn_gates* gt, const GdbTcBufs& b, int i, int cur,
                                 cudaStream_t st);
@@ -177,12 +175,6 @@ GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter) {
   return lo;
 }
 
-#define GDB_LAUNCH(expr, what)                                                                   \
-  do {                                                                                           \
-    cudaError_t _le = (expr);                                                                    \
-    if (_le != cudaSuccess) { set_error("%s launch: %s", what, cudaGetErrorString(_le)); return ICNN_E_CUDA; } \
-  } while (0)
-
 // The buffers of the tensor-core GEMMs of one iteration, with the optional epilogue accumulations / stores.
 static GdbTcBufs gdb_tc_bufs(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo,
                              const GdbAcc* acc, int store_it, float store_kappa) {
@@ -237,11 +229,11 @@ int gdb_forward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbL
     a.A0 = i ? ws + lo.Z[i - 1] : nullptr; a.G0 = i ? gt->cz[i] : nullptr; a.lda0 = a.K0;
     a.A1 = y; a.G1 = gt->cy[i]; a.lda1 = n; a.a1_scale = 1.f; a.a1_shift = 0.f;
     a.W = h->Wcat[i]; a.ldw = a.N; a.D = gt->d[i]; a.Z = ws + lo.Z[i]; a.alpha = h->alpha;
-    GDB_LAUNCH(launch_gemm<0>(a, st), "gd_backward forward");
+    ICNN_LAUNCH_CHECK(launch_gemm<0>(a, st), "gd_backward forward");
     if (tangent) {   // tangent layer: same product on (zt_{i-1}, a), pattern of Z_i, no bias
       a.A0 = i ? ws + lo.Zt[i - 1] : nullptr; a.A1 = av; a.D = nullptr;
       a.Zmask = ws + lo.Z[i]; a.Z = ws + lo.Zt[i];
-      GDB_LAUNCH(launch_gemm<2>(a, st), "gd_backward tangent");
+      ICNN_LAUNCH_CHECK(launch_gemm<2>(a, st), "gd_backward tangent");
     }
   }
   if (acc && acc->c)   // train_grad: the backward accumulates with c o Z_l + Zt_l in place of the tangent
@@ -274,7 +266,7 @@ int gdb_backward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gdb
     w.M = sl; w.N = 1; w.Kb = B; w.A = zt(L - 1); w.G = gt->cz[L]; w.lda = sl; w.D = acc->dL; w.ldd = 1;
     w.C = acc->gr->dWz[L]; w.ldc = 1; w.kappa = kp; w.C64 = acc->w64 ? acc->w64->dWz[L] : nullptr;
     w.part = ws + lo.wpart;
-    GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(L)");
+    ICNN_LAUNCH_CHECK(launch_wgrad(w, st), "gd_backward wgrad(L)");
   }
   int cur = 0;
   for (int i = L - 1; i >= 0; --i) {
@@ -283,7 +275,7 @@ int gdb_backward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gdb
       w.M = h->prev(i); w.N = h->hidden[i]; w.Kb = B; w.A = zt(i - 1); w.G = gt->cz[i]; w.lda = w.M;
       w.D = dl[cur]; w.ldd = w.N; w.C = acc->gr->dWz[i]; w.ldc = w.N; w.kappa = acc->kappa;
       w.C64 = acc->w64 ? acc->w64->dWz[i] : nullptr; w.part = ws + lo.wpart;
-      GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad");
+      ICNN_LAUNCH_CHECK(launch_wgrad(w, st), "gd_backward wgrad");
     }
     if (lo.use_tc) {
       int rc = picnn_gdb_tc_backward_layer(h, gt, tb, i, cur, st);
@@ -299,7 +291,7 @@ int gdb_backward(const icnn_picnn* h, const icnn_gates* gt, float* ws, const Gdb
     if (acc && i > 0) {
       a.dCz = acc->gr->dcz[i]; a.Ztprev = zt(i - 1); a.Dacc = ws + lo.Dacc[i - 1]; a.kappa = acc->kappa;
     }
-    GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward backward");
+    ICNN_LAUNCH_CHECK(launch_gemm<1>(a, st), "gd_backward backward");
     cur ^= 1;
   }
   return ICNN_OK;
@@ -314,20 +306,34 @@ int gdb_ygate_stage(const icnn_picnn* h, const icnn_gates* gt, float* ws, const 
     w.M = n; w.N = h->hidden[l]; w.Kb = B; w.A = av; w.G = gt->cy[l]; w.lda = n;
     w.D = ws + lo.Dacc[l]; w.ldd = w.N; w.C = gr->dWy[l]; w.ldc = w.N; w.kappa = 1.f;
     w.C64 = w64 ? w64->dWy[l] : nullptr; w.part = ws + lo.wpart;
-    GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy)");
+    ICNN_LAUNCH_CHECK(launch_wgrad(w, st), "gd_backward wgrad(Wy)");
     GemmArgs a{};   // dcy_l = a o (Delta_l Wy_l^T): the backward GEMM against the Wy rows of Wcat_l
     a.M = B; a.N0 = 0; a.N = n; a.K0 = h->hidden[l]; a.K1 = 0; a.A0 = ws + lo.Dacc[l]; a.lda0 = a.K0;
     a.W = h->Wcat[l] + (size_t)h->prev(l) * h->hidden[l]; a.ldw = a.K0; a.alpha = h->alpha;
     a.Cy = av; a.g = gr->dcy[l]; a.g_row_stride = n; a.n = n; a.g_scale = 1.f;
-    GDB_LAUNCH(launch_gemm<1>(a, st), "gd_backward dcy");
+    ICNN_LAUNCH_CHECK(launch_gemm<1>(a, st), "gd_backward dcy");
   }
   // output layer: Delta_L = ksum for every row (times dL[row] when given)
   WgradArgs w{};
   w.M = n; w.N = 1; w.Kb = B; w.A = av; w.G = gt->cy[L]; w.lda = n; w.D = dL; w.ldd = 1;
   w.C = gr->dWy[L]; w.ldc = 1; w.kappa = ksum; w.C64 = w64 ? w64->dWy[L] : nullptr; w.part = ws + lo.wpart;
-  GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
+  ICNN_LAUNCH_CHECK(launch_wgrad(w, st), "gd_backward wgrad(Wy_L)");
   rowbcast_fma_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(gr->dcy[L], av, h->Wcat[L] + h->hidden[L - 1], dL,
                                                                   ksum, N, n);
+  return ICNN_OK;
+}
+
+int gdb_check_args(const icnn_picnn* h, const icnn_gates* gates, const icnn_train_grads& gr, bool need_dd,
+                   const char* entry) {
+  ICNN_REQUIRE(gr.dWy && gr.dWz && gr.dcy && gr.dcz && (!need_dd || gr.dd), "null gradient array");
+  ICNN_REQUIRE(gates->B > 0, "empty batch");
+  if (gates->in_scale != 1.f || gates->in_shift != 0.f || gates->g_scale != 1.f) {
+    set_error("%s: the affine (RL) input wrapper is not on this path", entry);
+    return ICNN_E_UNSUPPORTED;
+  }
+  for (int l = 0; l <= h->L; ++l)
+    ICNN_REQUIRE(gr.dWy[l] && gr.dcy[l] && (!need_dd || gr.dd[l]) && (l == 0 || (gr.dWz[l] && gr.dcz[l])),
+                 "null gradient buffer");
   return ICNN_OK;
 }
 
@@ -344,14 +350,10 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
                                 const float* trueY, float loss_scale, int32_t nIter, float lr, float momentum,
                                 float* yN, const icnn_gd_grads* gr, void* workspace, void* stream) {
   ICNN_REQUIRE(h && gates && y0 && trueY && yN && gr && workspace, "null pointer");
-  ICNN_REQUIRE(gates->B > 0 && nIter >= 0, "empty batch or nIter < 0");
-  if (gates->in_scale != 1.f || gates->in_shift != 0.f || gates->g_scale != 1.f) {
-    set_error("icnn_gd_backward: the affine (RL) input wrapper is not on this path");
-    return ICNN_E_UNSUPPORTED;
-  }
+  ICNN_REQUIRE(nIter >= 0, "nIter < 0");
+  if (const int rc = gdb_check_args(h, gates, {gr->dWy, gr->dWz, gr->dcy, gr->dcz, nullptr}, false, "icnn_gd_backward"))
+    return rc;
   const int B = gates->B, n = h->n, L = h->L;
-  for (int l = 0; l <= L; ++l)
-    ICNN_REQUIRE(gr->dWy[l] && gr->dcy[l] && (l == 0 || (gr->dWz[l] && gr->dcz[l])), "null gradient buffer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const GdbLayout lo = gdb_layout(h, B, nIter);
   float* ws = static_cast<float*>(workspace);
@@ -394,7 +396,7 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
       a.M = B; a.N = h->hidden[l]; a.K0 = 0; a.K1 = n; a.A1 = av; a.G1 = gates->cy[l]; a.lda1 = n;
       a.a1_scale = 1.f; a.a1_shift = 0.f; a.W = h->Wcat[l] + (size_t)h->prev(l) * h->hidden[l]; a.ldw = a.N;
       a.Zmask = nullptr; a.Z = ws + lo.Ty[l]; a.alpha = h->alpha;
-      GDB_LAUNCH(launch_gemm<2>(a, st), "gd_backward Ty");
+      ICNN_LAUNCH_CHECK(launch_gemm<2>(a, st), "gd_backward Ty");
     }
     for (int l = 1; l <= L; ++l) {
       const int sp = h->prev(l);
@@ -423,7 +425,7 @@ extern "C" int icnn_gd_backward(const icnn_picnn_t* h, const icnn_gates* gates, 
         w.C = gr->dWz[L]; w.ldc = 1; w.kappa = 1.f;
       }
       w.part = ws + lo.wpart;
-      GDB_LAUNCH(launch_wgrad(w, st), "gd_backward wgrad (stored)");
+      ICNN_LAUNCH_CHECK(launch_wgrad(w, st), "gd_backward wgrad (stored)");
     }
   } else
   for (int pass = 0; pass < 2; ++pass) {

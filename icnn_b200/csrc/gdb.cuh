@@ -28,6 +28,24 @@ struct GdbW64 { double* dWy[ICNN_MAX_LAYERS + 1]; double* dWz[ICNN_MAX_LAYERS + 
 // caller scales delta_{L-1} by dL between gdb_forward and gdb_backward (dL depends on f).
 struct GdbAcc { const icnn_gd_grads* gr; float kappa; const float* c; const GdbW64* w64; const float* dL = nullptr; };
 
+// The argument checks of the FC training entries (icnn_gd_backward, icnn_train_grad, icnn_td_grad): no affine (RL)
+// input wrapper, a non-empty batch, and every per-layer gradient buffer the layers use (dd only with need_dd).
+// ICNN_OK, or the error code with the error set; entry names the entry point in the message.
+int gdb_check_args(const icnn_picnn* h, const icnn_gates* gates, const icnn_train_grads& gr, bool need_dd,
+                   const char* entry);
+
+// The float64 weight-gradient accumulators (train_grad.cu, td_grad.cu): dWy_0..L, then dWz_1..L, in one buffer of
+// gdb_w64_doubles(h) doubles.  gdb_w64_bind points a GdbW64 into it and zeroes it on st; gdb_w64_round writes the
+// sums, rounded once, into the float32 dWy / dWz of gr.
+size_t gdb_w64_doubles(const icnn_picnn* h);
+int gdb_w64_bind(const icnn_picnn* h, double* base, GdbW64* w, cudaStream_t st);
+int gdb_w64_round(const icnn_picnn* h, const GdbW64& w, const icnn_train_grads* gr, cudaStream_t st);
+
+// tensor-core buffers of the GD training backward (picnn_tc.cu): their floats for a B-row batch, with b's pointers
+// set from base when b != nullptr; and the (a o cy_l) columns of the tangent operands
+size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* base);
+void picnn_gdb_tc_gate_a(const icnn_picnn* h, const icnn_gates* gt, const float* a, const GdbTcBufs& b, cudaStream_t st);
+
 bool gdb_use_tc(const icnn_picnn* h, int B);
 GdbLayout gdb_layout(const icnn_picnn* h, int B, int nIter);
 int gdb_iteration(const icnn_picnn* h, const icnn_gates* gt, float* ws, const GdbLayout& lo, const GdbAcc* acc,

@@ -20,18 +20,15 @@
 // gdb_ygate_stage adds the y-gate terms.  dWy / dWz are summed in float64 (GdbW64) and rounded once; the loss is a
 // fixed-order float64 sum.  No atomics: every call gives the same bits.
 #include "gdb.cuh"
-#include "train_rows.cuh"
 #include "wgrad.cuh"
 
 namespace icnn {
-
-size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* base);
 
 constexpr int TD_MAX_B = 65536;          // the C4 minibatch; the whole batch runs as one block of rows
 constexpr int TD_LOSS_THREADS = 1024;
 
 struct TdLayout {
-  size_t w64, n64;   // bytes / doubles: float64 accumulators of dWy_0..L, dWz_1..L (in that order)
+  size_t w64;        // bytes: the float64 weight-gradient accumulators (gdb_w64_bind)
   size_t c;          // bytes: c [B] floats
   size_t gdb;        // bytes: gdb_layout(h, B, 0) floats from here
   GdbLayout lo;
@@ -42,8 +39,7 @@ static TdLayout td_layout(const icnn_picnn* h, int B) {
   TdLayout t{};
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
   size_t bytes = 0;
-  for (int l = 0; l <= h->L; ++l) t.n64 += (size_t)h->width(l) * (h->n + h->prev(l));
-  t.w64 = bytes; bytes += al(sizeof(double) * t.n64);
+  t.w64 = bytes; bytes += al(sizeof(double) * gdb_w64_doubles(h));
   t.c = bytes; bytes += al(sizeof(float) * (size_t)B);
   t.gdb = bytes;
   t.lo = gdb_layout(h, B, 0);
@@ -128,35 +124,21 @@ extern "C" int icnn_td_grad(const icnn_picnn_t* h, const icnn_gates* gates, cons
                             double* loss, const icnn_train_grads* gr, void* workspace, void* stream) {
   ICNN_REQUIRE(h && gates && act && negq_target && act2 && rew && term && td && loss && gr && workspace,
                "null pointer");
-  ICNN_REQUIRE(gr->dWy && gr->dWz && gr->dcy && gr->dcz && gr->dd, "null gradient array");
-  ICNN_REQUIRE(gates->B > 0, "empty batch");
+  if (const int rc = gdb_check_args(h, gates, *gr, true, "icnn_td_grad")) return rc;
   if (gates->B > TD_MAX_B) {
     set_error("icnn_td_grad: B = %d is above %d; split the minibatch", gates->B, TD_MAX_B);
     return ICNN_E_INVALID;
   }
-  if (gates->in_scale != 1.f || gates->in_shift != 0.f || gates->g_scale != 1.f) {
-    set_error("icnn_td_grad: the affine (RL bundle) input wrapper is not on this path; bind obs without it");
-    return ICNN_E_UNSUPPORTED;
-  }
   const int B = gates->B, n = h->n, L = h->L;
-  for (int l = 0; l <= L; ++l)
-    ICNN_REQUIRE(gr->dWy[l] && gr->dcy[l] && gr->dd[l] && (l == 0 || (gr->dWz[l] && gr->dcz[l])),
-                 "null gradient buffer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const TdLayout t = td_layout(h, B);
   const GdbLayout& lo = t.lo;
   char* wsb = static_cast<char*>(workspace);
   float* c = reinterpret_cast<float*>(wsb + t.c);
   float* ws = reinterpret_cast<float*>(wsb + t.gdb);
-  double* acc64 = reinterpret_cast<double*>(wsb + t.w64);
-  GdbW64 w64{};
-  {
-    size_t o = 0;
-    for (int l = 0; l <= L; ++l) { w64.dWy[l] = acc64 + o; o += (size_t)n * h->width(l); }
-    for (int l = 1; l <= L; ++l) { w64.dWz[l] = acc64 + o; o += (size_t)h->prev(l) * h->width(l); }
-  }
   // accumulated outputs and accumulators start from zero (dWy / dWz and dd are written whole at the end)
-  ICNN_CUDA_CHECK(cudaMemsetAsync(acc64, 0, sizeof(double) * t.n64, st));
+  GdbW64 w64;
+  if (const int rc = gdb_w64_bind(h, reinterpret_cast<double*>(wsb + t.w64), &w64, st)) return rc;
   for (int l = 0; l <= L; ++l) {
     ICNN_CUDA_CHECK(cudaMemsetAsync(gr->dcy[l], 0, sizeof(float) * (size_t)B * n, st));
     if (l > 0) ICNN_CUDA_CHECK(cudaMemsetAsync(gr->dcz[l], 0, sizeof(float) * (size_t)B * h->prev(l), st));
@@ -193,11 +175,5 @@ extern "C" int icnn_td_grad(const icnn_picnn_t* h, const icnn_gates* gates, cons
     ICNN_CUDA_CHECK(cudaMemcpyAsync(gr->dd[l], ws + lo.Dacc[l], sizeof(float) * (size_t)B * h->width(l),
                                     cudaMemcpyDeviceToDevice, st));
   ICNN_CUDA_CHECK(cudaMemcpyAsync(gr->dd[L], c, sizeof(float) * (size_t)B, cudaMemcpyDeviceToDevice, st));
-  for (int l = 0; l <= L; ++l) {
-    const long long Ny = (long long)n * h->width(l), Nz = (long long)h->prev(l) * h->width(l);
-    round_to_float_kernel<<<(unsigned)((Ny + 255) / 256), 256, 0, st>>>(gr->dWy[l], w64.dWy[l], Ny);
-    if (l > 0) round_to_float_kernel<<<(unsigned)((Nz + 255) / 256), 256, 0, st>>>(gr->dWz[l], w64.dWz[l], Nz);
-  }
-  ICNN_CUDA_CHECK(cudaGetLastError());
-  return ICNN_OK;
+  return gdb_w64_round(h, w64, gr, st);
 }

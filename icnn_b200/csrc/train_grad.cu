@@ -29,12 +29,9 @@
 
 namespace icnn {
 
-void picnn_gdb_tc_gate_a(const icnn_picnn* h, const icnn_gates* gt, const float* a, const GdbTcBufs& b, cudaStream_t st);
-size_t picnn_gdb_tc_ws_floats(const icnn_picnn* h, int B, GdbTcBufs* b, float* base);
-
 struct TgLayout {
   size_t off, row_u;          // bytes: device copy of row_offsets, row -> sample map
-  size_t w64, n64;            // bytes / doubles: float64 accumulators of dWy_0..L, dWz_1..L (in that order)
+  size_t w64;                 // bytes: the float64 weight-gradient accumulators (gdb_w64_bind)
   size_t gdb;                 // bytes: gdb_layout(h, cap, 0) floats from here
   GdbLayout lo;
   size_t cy[ICNN_MAX_LAYERS + 1], cz[ICNN_MAX_LAYERS + 1], d[ICNN_MAX_LAYERS + 1];   // per-row gates (floats)
@@ -70,9 +67,7 @@ static TgLayout tg_layout(const icnn_picnn* h, int B, long long R) {
   size_t bytes = 0;
   t.off = bytes; bytes += al(sizeof(long long) * ((size_t)B + 1));
   t.row_u = bytes; bytes += al(sizeof(int) * (size_t)t.cap);
-  t.n64 = 0;
-  for (int l = 0; l <= h->L; ++l) t.n64 += (size_t)h->width(l) * (h->n + h->prev(l));
-  t.w64 = bytes; bytes += al(sizeof(double) * t.n64);
+  t.w64 = bytes; bytes += al(sizeof(double) * gdb_w64_doubles(h));
   t.gdb = bytes;
   if (t.cap > 0) {
     t.lo = gdb_layout(h, (int)t.cap, 0);
@@ -87,11 +82,30 @@ static TgLayout tg_layout(const icnn_picnn* h, int B, long long R) {
   return t;
 }
 
-#define TG_LAUNCH(what)                                                                           \
-  do {                                                                                            \
-    cudaError_t _le = cudaGetLastError();                                                         \
-    if (_le != cudaSuccess) { set_error("train_grad %s: %s", what, cudaGetErrorString(_le)); return ICNN_E_CUDA; } \
-  } while (0)
+size_t gdb_w64_doubles(const icnn_picnn* h) {
+  size_t n64 = 0;
+  for (int l = 0; l <= h->L; ++l) n64 += (size_t)h->width(l) * (h->n + h->prev(l));
+  return n64;
+}
+
+int gdb_w64_bind(const icnn_picnn* h, double* base, GdbW64* w, cudaStream_t st) {
+  ICNN_CUDA_CHECK(cudaMemsetAsync(base, 0, sizeof(double) * gdb_w64_doubles(h), st));
+  *w = GdbW64{};
+  size_t o = 0;
+  for (int l = 0; l <= h->L; ++l) { w->dWy[l] = base + o; o += (size_t)h->n * h->width(l); }
+  for (int l = 1; l <= h->L; ++l) { w->dWz[l] = base + o; o += (size_t)h->prev(l) * h->width(l); }
+  return ICNN_OK;
+}
+
+int gdb_w64_round(const icnn_picnn* h, const GdbW64& w, const icnn_train_grads* gr, cudaStream_t st) {
+  for (int l = 0; l <= h->L; ++l) {
+    const long long Ny = (long long)h->n * h->width(l), Nz = (long long)h->prev(l) * h->width(l);
+    round_to_float_kernel<<<(unsigned)((Ny + 255) / 256), 256, 0, st>>>(gr->dWy[l], w.dWy[l], Ny);
+    if (l > 0) round_to_float_kernel<<<(unsigned)((Nz + 255) / 256), 256, 0, st>>>(gr->dWz[l], w.dWz[l], Nz);
+  }
+  ICNN_CUDA_CHECK(cudaGetLastError());
+  return ICNN_OK;
+}
 
 }  // namespace icnn
 
@@ -106,21 +120,10 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
                                const float* Y, const float* V, const float* c, const icnn_train_grads* gr,
                                void* workspace, void* stream) {
   ICNN_REQUIRE(h && gates && row_offsets && gr && workspace, "null pointer");
-  ICNN_REQUIRE(gr->dWy && gr->dWz && gr->dcy && gr->dcz && gr->dd, "null gradient array");
-  ICNN_REQUIRE(gates->B > 0, "empty batch");
-  if (gates->in_scale != 1.f || gates->in_shift != 0.f || gates->g_scale != 1.f) {
-    set_error("icnn_train_grad: the affine (RL) input wrapper is not on this path");
-    return ICNN_E_UNSUPPORTED;
-  }
+  if (const int rc = gdb_check_args(h, gates, *gr, true, "icnn_train_grad")) return rc;
   const int B = gates->B, n = h->n, L = h->L;
-  ICNN_REQUIRE(row_offsets[0] == 0, "row_offsets[0] != 0");
-  for (int u = 0; u < B; ++u) ICNN_REQUIRE(row_offsets[u + 1] >= row_offsets[u], "row_offsets decreasing");
-  const long long R = row_offsets[B];
-  ICNN_REQUIRE(R <= INT32_MAX, "more than 2^31 - 1 rows");
-  ICNN_REQUIRE(R == 0 || (Y && V && c), "null row input");
-  for (int l = 0; l <= L; ++l)
-    ICNN_REQUIRE(gr->dWy[l] && gr->dcy[l] && gr->dd[l] && (l == 0 || (gr->dWz[l] && gr->dcz[l])),
-                 "null gradient buffer");
+  const long long R = check_row_offsets(row_offsets, B, Y && V && c);
+  if (R < 0) return (int)R;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   for (int l = 0; l <= L; ++l) {   // outputs: accumulated over the chunks from zero
@@ -142,14 +145,8 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
   float* ws = reinterpret_cast<float*>(wsb + t.gdb);
   // (pageable source: the call returns once the offsets have been staged)
   ICNN_CUDA_CHECK(cudaMemcpyAsync(off_d, row_offsets, sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, st));
-  double* acc64 = reinterpret_cast<double*>(wsb + t.w64);
-  ICNN_CUDA_CHECK(cudaMemsetAsync(acc64, 0, sizeof(double) * t.n64, st));
-  GdbW64 w64{};
-  {
-    size_t o = 0;
-    for (int l = 0; l <= L; ++l) { w64.dWy[l] = acc64 + o; o += (size_t)n * h->width(l); }
-    for (int l = 1; l <= L; ++l) { w64.dWz[l] = acc64 + o; o += (size_t)h->prev(l) * h->width(l); }
-  }
+  GdbW64 w64;
+  if (const int rc = gdb_w64_bind(h, reinterpret_cast<double*>(wsb + t.w64), &w64, st)) return rc;
 
   // per-row views of the chunk: gates and the gate-adjoint outputs of gdb_iteration
   float *cy[ICNN_MAX_LAYERS + 1], *cz[ICNN_MAX_LAYERS + 1], *dd[ICNN_MAX_LAYERS + 1];
@@ -173,17 +170,17 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
     GdbLayout lo = t.lo;
     lo.use_tc = lo.use_tc && gdb_use_tc(h, rows);
     gt.B = rows;
-    row_sample_kernel<<<cdiv(rows, 256), 256, 0, st>>>(row_u, off_d, u0, u1, r0, rows);
+    launch_row_sample(row_u, off_d, u0, u1, r0, rows, st);
     for (int l = 0; l <= L; ++l) {
       const long long Nn = (long long)rows * n, Nd = (long long)rows * h->width(l), Nz = (long long)rows * h->prev(l);
-      gather_rows_kernel<<<(unsigned)((Nn + 255) / 256), 256, 0, st>>>(cy[l], gates->cy[l], row_u, Nn, n);
-      gather_rows_kernel<<<(unsigned)((Nd + 255) / 256), 256, 0, st>>>(dd[l], gates->d[l], row_u, Nd, h->width(l));
-      if (l > 0) gather_rows_kernel<<<(unsigned)((Nz + 255) / 256), 256, 0, st>>>(cz[l], gates->cz[l], row_u, Nz, h->prev(l));
+      launch_gather_rows(cy[l], gates->cy[l], row_u, rows, n, st);
+      launch_gather_rows(dd[l], gates->d[l], row_u, rows, h->width(l), st);
+      if (l > 0) launch_gather_rows(cz[l], gates->cz[l], row_u, rows, h->prev(l), st);
       ICNN_CUDA_CHECK(cudaMemsetAsync(dcy[l], 0, sizeof(float) * Nn, st));
       if (l > 0) ICNN_CUDA_CHECK(cudaMemsetAsync(dcz[l], 0, sizeof(float) * Nz, st));
       if (l < L) ICNN_CUDA_CHECK(cudaMemsetAsync(ws + lo.Dacc[l], 0, sizeof(float) * Nd, st));
     }
-    TG_LAUNCH("gather");
+    ICNN_LAUNCH_CHECK(cudaGetLastError(), "train_grad gather");
     ICNN_CUDA_CHECK(cudaMemcpyAsync(ws + lo.y, Y + r0 * n, sizeof(float) * rows * n, cudaMemcpyDeviceToDevice, st));
     ICNN_CUDA_CHECK(cudaMemcpyAsync(ws + lo.a, V + r0 * n, sizeof(float) * rows * n, cudaMemcpyDeviceToDevice, st));
     if (lo.use_tc) {   // the (v o cy_l) columns of the tangent operands
@@ -199,26 +196,18 @@ extern "C" int icnn_train_grad(const icnn_picnn_t* h, const icnn_gates* gates, c
     if (rc) return rc;
 
     // per-row gate adjoints -> per-sample outputs; dd_l = sum_r c_r delta_l (delta_L = 1)
-    const long long NS = (long long)(u1 - u0);
     for (int l = 0; l <= L; ++l) {
       const int wl = h->width(l), pl = h->prev(l);
       const SegView one{nullptr, nullptr, 0, 1, 0, 0};
-      segsum_prod_kernel<<<(unsigned)((NS * n + 255) / 256), 256, 0, st>>>(
-          gr->dcy[l], SegView{dcy[l], nullptr, n, n, 0, 0}, one, nullptr, n, off_d, u0, u1, r0, r1);
+      launch_segsum_prod(gr->dcy[l], SegView{dcy[l], nullptr, n, n, 0, 0}, one, nullptr, n, off_d, u0, u1, r0, r1, st);
       if (l > 0)
-        segsum_prod_kernel<<<(unsigned)((NS * pl + 255) / 256), 256, 0, st>>>(
-            gr->dcz[l], SegView{dcz[l], nullptr, pl, pl, 0, 0}, one, nullptr, pl, off_d, u0, u1, r0, r1);
-      segsum_prod_kernel<<<(unsigned)((NS * wl + 255) / 256), 256, 0, st>>>(
-          gr->dd[l], l < L ? SegView{ws + lo.Dacc[l], nullptr, wl, wl, 0, 0} : one, one, c, wl, off_d, u0, u1, r0, r1);
+        launch_segsum_prod(gr->dcz[l], SegView{dcz[l], nullptr, pl, pl, 0, 0}, one, nullptr, pl, off_d, u0, u1, r0, r1,
+                           st);
+      launch_segsum_prod(gr->dd[l], l < L ? SegView{ws + lo.Dacc[l], nullptr, wl, wl, 0, 0} : one, one, c, wl, off_d,
+                         u0, u1, r0, r1, st);
     }
-    TG_LAUNCH("segmented sum");
+    ICNN_LAUNCH_CHECK(cudaGetLastError(), "train_grad segmented sum");
     r0 = r1;
   }
-  for (int l = 0; l <= L; ++l) {   // the float64 weight-gradient sums, rounded once
-    const long long Ny = (long long)n * h->width(l), Nz = (long long)h->prev(l) * h->width(l);
-    round_to_float_kernel<<<(unsigned)((Ny + 255) / 256), 256, 0, st>>>(gr->dWy[l], w64.dWy[l], Ny);
-    if (l > 0) round_to_float_kernel<<<(unsigned)((Nz + 255) / 256), 256, 0, st>>>(gr->dWz[l], w64.dWz[l], Nz);
-  }
-  ICNN_CUDA_CHECK(cudaGetLastError());
-  return ICNN_OK;
+  return gdb_w64_round(h, w64, gr, st);   // the float64 weight-gradient sums, rounded once
 }

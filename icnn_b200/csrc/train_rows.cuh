@@ -60,6 +60,35 @@ static __global__ void segsum_prod_kernel(float* out, SegView a, SegView e, cons
   out[(long long)u * w + j] = (float)((double)out[(long long)u * w + j] + acc);
 }
 
+// launches over one chunk (256 threads per block): rows rows from r0, samples [u0, u1)
+static inline void launch_row_sample(int* row_u, const long long* off, int u0, int u1, long long r0, int rows,
+                                     cudaStream_t st) {
+  row_sample_kernel<<<cdiv(rows, 256), 256, 0, st>>>(row_u, off, u0, u1, r0, rows);
+}
+// dst [rows, w] = the rows of src [B, w] of each chunk row's sample
+static inline void launch_gather_rows(float* dst, const float* src, const int* row_u, int rows, long long w,
+                                      cudaStream_t st) {
+  const long long N = (long long)rows * w;
+  gather_rows_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(dst, src, row_u, N, (int)w);
+}
+static inline void launch_segsum_prod(float* out, SegView a, SegView e, const float* scale, long long w,
+                                      const long long* off, int u0, int u1, long long r0, long long r1,
+                                      cudaStream_t st) {
+  const long long N = (long long)(u1 - u0) * w;
+  segsum_prod_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(out, a, e, scale, (int)w, off, u0, u1, r0, r1);
+}
+
+// The CSR row offsets of B > 0 samples: row_offsets[0] = 0, non-decreasing, at most 2^31 - 1 rows, and the row
+// inputs given (have_rows) when there are rows.  Returns R = row_offsets[B], or ICNN_E_INVALID with the error set.
+static inline long long check_row_offsets(const int64_t* row_offsets, int B, bool have_rows) {
+  ICNN_REQUIRE(row_offsets[0] == 0, "row_offsets[0] != 0");
+  for (int u = 0; u < B; ++u) ICNN_REQUIRE(row_offsets[u + 1] >= row_offsets[u], "row_offsets decreasing");
+  const long long R = row_offsets[B];
+  ICNN_REQUIRE(R <= INT32_MAX, "more than 2^31 - 1 rows");
+  ICNN_REQUIRE(R == 0 || have_rows, "null row input");
+  return R;
+}
+
 // rows per chunk: ICNN_TRAIN_CHUNK if set, else what fits ICNN_TRAIN_WS_GB (default 2) GiB at bytes_per_row
 // (at least 64, at most R)
 static inline long long chunk_rows(double bytes_per_row, long long R) {

@@ -26,8 +26,7 @@ import numpy as np
 import torch
 
 from . import _capi
-from .conv_picnn import (BoundConvPICNN, _gate_vjp, _to_host, _train_grad_buffers, _ypath_grads, conv_gd_trainable,
-                         conv_trainable)
+from .conv_picnn import BoundConvPICNN, _gate_vjp, _train_grad_buffers, _ypath_grads, conv_gd_trainable, conv_trainable
 from .picnn import BoundPICNN
 
 
@@ -35,6 +34,56 @@ def _f32(a, dev):
     if isinstance(a, torch.Tensor):
         return a.to(device=dev, dtype=torch.float32).contiguous()
     return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32), device=dev)
+
+
+def _host(v):
+    """Tensors, also inside lists and dicts, as numpy arrays (None stays None)."""
+    if isinstance(v, dict):
+        return {k: _host(t) for k, t in v.items()}
+    if isinstance(v, list):
+        return [_host(t) for t in v]
+    return None if v is None else v.cpu().numpy()
+
+
+def _check_fg(fg, who, x=None, conv=True):
+    """Refuses an ``fg`` the training gradient ``who`` does not take: anything but a ``BoundPICNN`` without the
+    affine RL wrapper or, with ``conv``, a ``BoundConvPICNN``.  Returns True for the latter, whose x-path uses the
+    minibatch it was bound to (so ``x`` is refused)."""
+    if conv and isinstance(fg, BoundConvPICNN):
+        if x is not None:
+            raise ValueError("%s: a BoundConvPICNN uses the minibatch it was bound to; do not pass x" % who)
+        return True
+    if not isinstance(fg, BoundPICNN):
+        raise TypeError("%s needs a BoundPICNN (PICNN.bind(x))%s"
+                        % (who, " or a BoundConvPICNN (ConvPICNN.bind(x))" if conv else ""))
+    if fg.affine:
+        raise ValueError("%s: the affine RL wrapper is not part of this training graph; bind without affine=True" % who)
+    return False
+
+
+def _check_shape(who, shape, **tensors):
+    """ValueError unless every one of the named ``tensors`` has ``shape``."""
+    if any(tuple(t.shape) != shape for t in tensors.values()):
+        raise ValueError("%s: %s must be %s, got %s" % (who, " and ".join(tensors), list(shape),
+                                                       " and ".join(str(tuple(t.shape)) for t in tensors.values())))
+
+
+def _grad_buffers(fg, dd=False):
+    """Output buffers of an FC training gradient for ``fg``'s batch: per-layer lists 'Wy', 'Wz', 'dcy', 'dcz' (and
+    'dd' with ``dd``), the host pointer arrays, and the C struct over them (``TrainGrads`` with ``dd``, else
+    ``GdGrads``).  The arrays must outlive the work."""
+    net, dev, B = fg.net, fg.net.device, fg.B
+    n, L, hid = net.n, net.L, net.hidden
+    width = lambda l: hid[l] if l < L else 1          # noqa: E731
+    prev = lambda l: hid[l - 1]                        # noqa: E731
+    z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+    grads = dict(Wy=[z(n, width(l)) for l in range(L + 1)], Wz=[None] + [z(prev(l), width(l)) for l in range(1, L + 1)],
+                 dcy=[z(B, n) for _ in range(L + 1)], dcz=[None] + [z(B, prev(l)) for l in range(1, L + 1)])
+    if dd:
+        grads["dd"] = [z(B, width(l)) for l in range(L + 1)]
+    arrs = [_capi.ptr_array(v) for v in grads.values()]
+    gr = (_capi.TrainGrads if dd else _capi.GdGrads)(*[C.cast(a, _capi._fpp) for a in arrs])
+    return grads, arrs, gr
 
 
 def gd_grad(fg: BoundPICNN, y0, trueY, nIter=30, lr=0.01, momentum=0.3, loss_scale=None, x=None,
@@ -52,76 +101,38 @@ def gd_grad(fg: BoundPICNN, y0, trueY, nIter=30, lr=0.01, momentum=0.3, loss_sca
     adjoints 'dcy' (per conv layer) and 'dcz' (per layer, [B, flat gate]).  The additive gates 'z{l}_u/*' and the
     y_red biases 'z{l}_y_red/b' are in gv_ with a gradient that is exactly zero, and are returned as zeros.  Numpy
     arrays, or with ``return_device=True`` torch tensors on the net's device (for ``net.vars[k].grad = g``)."""
-    if isinstance(fg, BoundConvPICNN):
-        if x is not None:
-            raise ValueError("gd_grad: a BoundConvPICNN uses the minibatch it was bound to; do not pass x")
-        return _conv_gd_grad(fg, y0, trueY, nIter, lr, momentum, loss_scale, return_device)
-    if not isinstance(fg, BoundPICNN):
-        raise TypeError("gd_grad needs a BoundPICNN (PICNN.bind(x)) or a BoundConvPICNN (ConvPICNN.bind(x))")
-    if fg.affine:
-        raise ValueError("gd_grad: the affine RL wrapper is not part of the icnn.back training graph")
-    net, dev, B = fg.net, fg.net.device, fg.B
-    n, L, hid = net.n, net.L, net.hidden
-    width = lambda l: hid[l] if l < L else 1          # noqa: E731
-    prev = lambda l: hid[l - 1]                        # noqa: E731
-    with torch.cuda.device(dev):
-        y0d, tY = _f32(y0, dev), _f32(trueY, dev)
-        assert tuple(y0d.shape) == (B, n) and tuple(tY.shape) == (B, n)
-        if loss_scale is None:
-            loss_scale = 2.0 / (B * n)
-        z = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-        dWy = [z(n, width(l)) for l in range(L + 1)]
-        dcy = [z(B, n) for _ in range(L + 1)]
-        dWz = [None] + [z(prev(l), width(l)) for l in range(1, L + 1)]
-        dcz = [None] + [z(B, prev(l)) for l in range(1, L + 1)]
-        yN = z(B, n)
-        arrs = [_capi.ptr_array(v) for v in (dWy, dWz, dcy, dcz)]
-        gr = _capi.GdGrads(*[C.cast(a, _capi._fpp) for a in arrs])
-        ws = torch.empty(max(_capi.lib.icnn_gd_backward_workspace_bytes(net._h, B, int(nIter)), 4), dtype=torch.uint8,
-                         device=dev)
-        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _capi.check(_capi.lib.icnn_gd_backward(net._h, C.byref(fg.c_gates), y0d.data_ptr(), tY.data_ptr(),
-                                               float(loss_scale), int(nIter), float(lr), float(momentum),
-                                               yN.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
-        grads = dict(Wy=dWy, Wz=dWz, dcy=dcy, dcz=dcz)
-        if x is not None:
-            grads.update(_xpath_backward(net, _f32(x, dev), dcy, dcz))
-        torch.cuda.current_stream().synchronize()      # ws / arrs stay alive until the work is done
-    if return_device:
-        return yN, grads
-    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
-    return host(yN), {k: [host(t) for t in v] for k, v in grads.items()}
-
-
-def _conv_gd_grad(fg, y0, trueY, nIter, lr, momentum, loss_scale, return_device):
+    conv = _check_fg(fg, "gd_grad", x)
     net, dev, B, n = fg.net, fg.net.device, fg.B, fg.net.n
     with torch.cuda.device(dev):
         y0d, tY = _f32(y0, dev), _f32(trueY, dev)
-        if tuple(y0d.shape) != (B, n) or tuple(tY.shape) != (B, n):
-            raise ValueError("gd_grad: y0 and trueY must be [%d, %d], got %s and %s"
-                             % (B, n, tuple(y0d.shape), tuple(tY.shape)))
+        _check_shape("gd_grad", (B, n), y0=y0d, trueY=tY)
         if loss_scale is None:
             loss_scale = 2.0 / (B * n)
-        o, gr, arrs = _train_grad_buffers(fg)
+        if conv:
+            o, gr, arrs = _train_grad_buffers(fg)
+            entry, ws_bytes = _capi.lib.icnn_conv_gd_backward, _capi.lib.icnn_conv_gd_backward_workspace_bytes
+        else:
+            grads, arrs, gr = _grad_buffers(fg)
+            entry, ws_bytes = _capi.lib.icnn_gd_backward, _capi.lib.icnn_gd_backward_workspace_bytes
         yN = torch.empty(B, n, dtype=torch.float32, device=dev)
-        ws = torch.empty(max(_capi.lib.icnn_conv_gd_backward_workspace_bytes(net._h, B, int(nIter)), 4),
-                         dtype=torch.uint8, device=dev)
-        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _capi.check(_capi.lib.icnn_conv_gd_backward(net._h, C.byref(fg.c_gates), y0d.data_ptr(), tY.data_ptr(),
-                                                    float(loss_scale), int(nIter), float(lr), float(momentum),
-                                                    yN.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
-        grads = _ypath_grads(net, o)
-        # x-path through the gates of the bound minibatch, over the same variables as the bundle-entropy mode (so
-        # that the two give the same bits on the same rows); dd is zero, and the output layer's additive gate,
-        # which only dd reaches, is then dropped
-        names = [k for k in conv_trainable(net) if k not in grads]
-        grads.update(_gate_vjp(fg, names, o["dcy"], o["dcz"], o["dd"]))
-        grads = {k: grads[k] for k in conv_gd_trainable(net)}
-        grads.update(dcy=o["dcy"], dcz=o["dcz"])
+        ws = _capi.workspace(ws_bytes(net._h, B, int(nIter)), dev)
+        _capi.check(entry(net._h, C.byref(fg.c_gates), y0d.data_ptr(), tY.data_ptr(), float(loss_scale), int(nIter),
+                          float(lr), float(momentum), yN.data_ptr(), C.byref(gr), ws.data_ptr(), _capi.stream()))
+        if conv:
+            grads = _ypath_grads(net, o)
+            # x-path through the gates of the bound minibatch, over the same variables as the bundle-entropy mode (so
+            # that the two give the same bits on the same rows); dd is zero, and the output layer's additive gate,
+            # which only dd reaches, is then dropped
+            names = [k for k in conv_trainable(net) if k not in grads]
+            grads.update(_gate_vjp(fg, names, o["dcy"], o["dcz"], o["dd"]))
+            grads = {k: grads[k] for k in conv_gd_trainable(net)}
+            grads.update(dcy=o["dcy"], dcz=o["dcz"])
+        elif x is not None:
+            grads.update(_xpath_backward(net, _f32(x, dev), grads["dcy"], grads["dcz"]))
         torch.cuda.current_stream().synchronize()      # ws / arrs stay alive until the work is done
     if return_device:
         return yN, grads
-    return yN.cpu().numpy(), _to_host(grads)
+    return _host(yN), _host(grads)
 
 
 def _xpath_backward(net, x, dcy, dcz, dd=None):

@@ -32,8 +32,7 @@ import numpy as np
 import torch
 
 from . import _capi
-from .bundle_grad import _grad_buffers
-from .gd_grad import _f32, _xpath_backward
+from .gd_grad import _check_fg, _check_shape, _f32, _grad_buffers, _host, _xpath_backward
 from .picnn import BoundPICNN
 
 # agent.py:13-15 (discount, l2norm) and tflearn's fully_connected default weight_decay
@@ -42,27 +41,19 @@ DISCOUNT, L2NORM, WEIGHT_DECAY = 0.99, 1e-4, 1e-3
 WEIGHTS = ("Wy", "Wz", "Wu", "Wzu", "Wyu", "Wzx")
 
 
-def _check(fg, who):
-    if not isinstance(fg, BoundPICNN):
-        raise TypeError("td_grad: %s must be a BoundPICNN (PICNN.bind(obs))" % who)
-    if fg.affine:
-        raise ValueError("td_grad: bind %s without affine=True: the TD step sees the action in [-1, 1]" % who)
-
-
 def _launch(fg, act, negq_t, act2, rew, term, discount):
     """icnn_td_grad on the current stream (asynchronous): (td, loss [1] float64, grads, what must outlive the work)."""
     net, dev, B = fg.net, fg.net.device, fg.B
-    grads, arrs, gr = _grad_buffers(fg)
+    grads, arrs, gr = _grad_buffers(fg, dd=True)
     td = torch.empty(B, dtype=torch.float32, device=dev)
     loss = torch.empty(1, dtype=torch.float64, device=dev)
     nbytes = _capi.lib.icnn_td_grad_workspace_bytes(net._h, B)
     if nbytes == 0:
         raise ValueError("td_grad: no workspace for B = %d (the library takes up to 65536 samples per call)" % B)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    ws = _capi.workspace(nbytes, dev)
     _capi.check(_capi.lib.icnn_td_grad(net._h, C.byref(fg.c_gates), act.data_ptr(), negq_t.data_ptr(), act2.data_ptr(),
                                        rew.data_ptr(), term.data_ptr(), float(discount), td.data_ptr(),
-                                       loss.data_ptr(), C.byref(gr), ws.data_ptr(), stream))
+                                       loss.data_ptr(), C.byref(gr), ws.data_ptr(), _capi.stream()))
     return td, loss, grads, (arrs, gr, ws)
 
 
@@ -80,8 +71,8 @@ def td_grad(fg: BoundPICNN, fg_target: BoundPICNN, obs, act, rew, act2, term, di
     per-layer lists like ``bundle_grad``) to d loss_q / d theta including the L2 term, and 'dcy', 'dcz', 'dd' to the
     per-sample gate adjoints of mean(td^2).  ``loss_q`` is a float and ``td`` [B] numpy; with ``return_device``
     ``loss_q`` is a 0-d float64 tensor and everything else torch tensors on the net's device."""
-    _check(fg, "fg")
-    _check(fg_target, "fg_target")
+    _check_fg(fg, "td_grad (fg)", conv=False)
+    _check_fg(fg_target, "td_grad (fg_target)", conv=False)
     net, dev, B, n = fg.net, fg.net.device, fg.B, fg.net.n
     if fg_target.B != B or fg_target.net.n != n or fg_target.net.device != dev:
         raise ValueError("td_grad: fg_target is for B=%d, n=%d on %s, fg for B=%d, n=%d on %s"
@@ -93,12 +84,8 @@ def td_grad(fg: BoundPICNN, fg_target: BoundPICNN, obs, act, rew, act2, term, di
             termd = term.to(device=dev, dtype=torch.bool).to(torch.uint8).reshape(-1).contiguous()
         else:
             termd = torch.as_tensor(np.asarray(term, dtype=bool).astype(np.uint8).reshape(-1), device=dev)
-        if tuple(actd.shape) != (B, n) or tuple(act2d.shape) != (B, n):
-            raise ValueError("td_grad: act and act2 must be [%d, %d], got %s and %s"
-                             % (B, n, tuple(actd.shape), tuple(act2d.shape)))
-        if tuple(obsd.shape) != (B, net.m):
-            raise ValueError("td_grad: obs must be the [%d, %d] minibatch fg was bound to, got %s"
-                             % (B, net.m, tuple(obsd.shape)))
+        _check_shape("td_grad", (B, n), act=actd, act2=act2d)
+        _check_shape("td_grad", (B, net.m), obs=obsd)      # the minibatch fg was bound to
         if rewd.shape[0] != B or termd.shape[0] != B:
             raise ValueError("td_grad: rew and term must have %d entries" % B)
         negq_t, _ = fg_target.fg_device(act2d)
@@ -122,5 +109,4 @@ def td_grad(fg: BoundPICNN, fg_target: BoundPICNN, obs, act, rew, act2, term, di
         del keep
     if return_device:
         return loss_q, td, grads
-    host = lambda v: None if v is None else v.cpu().numpy()   # noqa: E731
-    return float(loss_q), td.cpu().numpy(), {k: [host(t) for t in v] for k, v in grads.items()}
+    return float(loss_q), _host(td), _host(grads)
