@@ -7,12 +7,12 @@ The energy is restated from the reference's Model.f (completion/icnn_ebundle.py:
 into the x-path (per sample: the gates) and the y-path (per row, given its sample's gates), so that the gate
 adjoints are gradients with respect to the gate tensors themselves.  tests/test_conv_train_grad_golden_cpu.py pins
 its gradient and variable set to the reference's own training step (tests/golden/conv/conv_train_grad.npz);
-tests/test_conv_train_grad_cpu.py pins its energy to tests/conv_energy.energy and its gradient to central finite
+tests/test_conv_train_grad_cpu.py pins its energy to oracle/conv_energy.energy and its gradient to central finite
 differences."""
 import numpy as np
 import torch
 
-from icnn_b200.conv_picnn import _same_conv
+from oracle.conv_picnn import same_conv_tf as _same_conv
 
 BN_STATS = ("moving_mean", "moving_variance")
 
@@ -26,7 +26,7 @@ def trainable(names, Lc, Ld):
 
 def make_variables(H, W, convs, fcs, seed=0, bn=True):
     """Random variables of the completion Model in TensorFlow names and layouts (conv kernels [k, k, c_in, c_out],
-    dense [in, out] on the NHWC-flattened map), scaled like tests/conv_picnn.py; with ``bn`` non-identity
+    dense [in, out] on the NHWC-flattened map), scaled like oracle/conv_picnn.py; with ``bn`` non-identity
     inference batch-norm statistics and affine parameters."""
     rs = np.random.RandomState(seed)
     rnd = lambda *s, fan: rs.randn(*s) / np.sqrt(fan)          # noqa: E731

@@ -10,31 +10,17 @@ The PICNN f/g callback they are fed is oracle/picnn_np.py (the reference's own f
 TensorFlow graph and TensorFlow is not installed) in float64; inputs are regenerated from the
 seed by oracle/synth.py, and a checksum of the inputs is stored so generator drift is caught.
 
-Usage:  python oracle/gen_golden.py [case ...]
+Usage:  python -m oracle.gen_golden [case ...]      -> tests/golden/<case>.npz
 """
-import contextlib
 import hashlib
-import importlib.util
-import io
-import os
 import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from oracle import picnn_np, synth  # noqa: E402
+from oracle import picnn_np, refcode, regen, synth
 
-REF = os.environ.get("ICNN_REFERENCE_DIR", "")
-
-
-def _load(name, path):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
+GOLDEN = "%s.npz"        # % case name
 
 # (case name, config, B, nIter, variant, solver)
 CASES = [
@@ -74,25 +60,27 @@ def pack_ragged(lst, kmax, inner_shape, dtype=np.float64):
     return out
 
 
-def compute_case(name, cfgname, B, nIter, variant, solver):
-    """-> (arrays of the golden file, seconds, counts, nIters): the UNMODIFIED reference module run on the seeded case."""
+def generate(name):
+    """-> the arrays of tests/golden/<name>.npz: the UNMODIFIED reference module run on the seeded case."""
+    _, cfgname, B, nIter, variant, solver = next(c for c in CASES if c[0] == name)
     cfg = synth.CONFIGS[cfgname]
     p, x, y0 = synth.make_inputs(cfgname, B=B)
     fg = picnn_np.make_fg(p, x, affine=cfg["affine"])
     if variant == "lib":
-        mod = _load("ref_pc", os.path.join(REF, "lib/bundle_entropy.py"))
+        mod = refcode.load("ref_pc", "lib/bundle_entropy.py")
         call = lambda: mod.solveBatch(fg, y0.copy(), nIter=nIter, solver=solver)  # noqa: E731
     elif variant == "dual":
-        mod = _load("ref_dual", os.path.join(REF, "lib/bundle_entropy_dual.py"))
+        mod = refcode.load("ref_dual", "lib/bundle_entropy_dual.py")
         call = lambda: mod.solveBatch(fg, y0.copy(), nIter=nIter)  # noqa: E731
     else:
-        mod = _load("ref_rl", os.path.join(REF, "RL/src/bundle_entropy.py"))
+        mod = refcode.load("ref_rl", "RL/src/bundle_entropy.py")
         call = lambda: mod.solveBatch(fg, y0.copy(), nIter=nIter)  # noqa: E731
     t0 = time.time()
-    with contextlib.redirect_stdout(io.StringIO()), np.errstate(all="ignore"):
+    with refcode.quiet():
         xf, A, b, lam, xs, nIters = call()
-    dt = time.time() - t0
     counts = np.array([len(a) for a in A], dtype=np.int32)
+    print("%-12s %-3s B=%-4d nIter=%-3d %-4s  %.1fs  k mean %.2f max %d  nIters mean %.2f" % (
+        name, cfgname, B, nIter, variant, time.time() - t0, counts.mean(), counts.max(), np.mean(nIters)))
     kmax = max(1, int(counts.max()))
     n = cfg["n"]
     out = dict(
@@ -105,20 +93,8 @@ def compute_case(name, cfgname, B, nIter, variant, solver):
     if n <= 512:  # keep fixtures small: rows / iterates only for the small shapes
         out["A"] = pack_ragged(A, kmax, (n,))
         out["xs"] = pack_ragged(xs, kmax, (n,))
-    return out, dt, counts, nIters
-
-
-def run_case(name, cfgname, B, nIter, variant, solver):
-    out, dt, counts, nIters = compute_case(name, cfgname, B, nIter, variant, solver)
-    path = os.path.join(ROOT, "tests", "golden", name + ".npz")
-    np.savez_compressed(path, **out)
-    print("%-12s %-3s B=%-4d nIter=%-3d %-4s  %.1fs  k mean %.2f max %d  nIters mean %.2f  -> %s (%d KB)" % (
-        name, cfgname, B, nIter, variant, dt, counts.mean(), counts.max(), np.mean(nIters), path,
-        os.path.getsize(path) // 1024))
+    return out
 
 
 if __name__ == "__main__":
-    want = set(sys.argv[1:])
-    for case in CASES:
-        if not want or case[0] in want:
-            run_case(*case)
+    regen.main(("gen_golden",), only=[GOLDEN % c for c in sys.argv[1:]])

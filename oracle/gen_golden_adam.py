@@ -2,50 +2,31 @@
 """Golden vectors for the RL Adam argmin from the reference's own `Agent.adam` body
 (RL/src/icnn.py:160-215; the module imports TensorFlow, so the method source is cut out with ast
 and exec'd with a stub `self`).  func = oracle fg_entr on the C4 (HalfCheetah) dims.
-TEST INFRASTRUCTURE ONLY; runs in the build container only."""
-import ast
-import contextlib
-import io
-import os
-import sys
+TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
+Usage:  python -m oracle.gen_golden_adam   -> tests/golden/adam.npz"""
 import types
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from oracle import adam_np, synth  # noqa: E402
-from oracle.gen_golden import REF  # noqa: E402
+from oracle import adam_np, refcode, regen, synth
+
+GOLDEN = "adam.npz"
 
 
-def extract_method(path, cls, name):
-    tree = ast.parse(open(path).read())
-    for node in tree.body:
-        if isinstance(node, ast.ClassDef) and node.name == cls:
-            for sub in node.body:
-                if isinstance(sub, ast.FunctionDef) and sub.name == name:
-                    ns = {"np": np}
-                    exec(compile(ast.Module(body=[sub], type_ignores=[]), path, "exec"), ns)
-                    return ns[name]
-    raise KeyError(name)
-
-
-def main():
-    adam = extract_method(os.path.join(REF, "RL/src/icnn.py"), "Agent", "adam")
+def generate():
+    adam = refcode.extract("RL/src/icnn.py", ["Agent.adam"], {"np": np})["adam"]
     out = {}
     for tag, B in (("c4", 96),):
         p, x, _ = synth.make_inputs("C4", B=B)
         func = adam_np.make_fg_entr(p, x)
         stub = types.SimpleNamespace(dimA=p.n)
-        with contextlib.redirect_stdout(io.StringIO()) as buf:
+        with refcode.quiet() as buf:
             best = adam(stub, func, x)
         its = [int(s.split()[3]) for s in buf.getvalue().splitlines() if "Adam took" in s]
         out[tag + "_act_best"] = best
         out[tag + "_iters"] = np.array(its[-1] if its else 1000)
-    path = os.path.join(ROOT, "tests", "golden", "adam.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, {k: (v.shape if hasattr(v, "shape") else v) for k, v in out.items()}, out["c4_iters"])
+    return out
 
 
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_adam",))

@@ -13,18 +13,18 @@ that sample's rows, so every gradient is stored per sample ([B, ...]): every arr
 at most 4096 entries at C3.  Weights and x are regenerated from seeds by ``case_inputs`` (shared with the tests).
 
 TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
-Usage:  python oracle/gen_golden_bundle_grad.py
+Usage:  python -m oracle.gen_golden_bundle_grad   -> tests/golden/training/bundle_grad.npz
 """
-import contextlib
-import io
-import os
-import sys
+import types
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from icnn_b200 import workloads  # noqa: E402  (pure-numpy input generator)
+from icnn_b200 import workloads  # (pure-numpy input generator)
+from oracle import picnn_np, refcode, regen
+from oracle.tf_shim import Shim, variables_from_params
+
+# a subdirectory: tests/test_oracle_golden.py runs every tests/golden/*.npz as a solveBatch case
+GOLDEN = "training/bundle_grad.npz"
 
 # tag -> (B, nIter, layerSizes passed to Model; the Model appends nLabels)
 CASES = {"small": (12, 8, [14, 11]), "c3": (6, 10, [600])}
@@ -57,7 +57,7 @@ def case_inputs(tag):
 
 
 def tf_name_to_param(name):
-    """'z1_yu/W' -> ('Wy', 1) etc. (oracle/gen_golden_tfshim.variables_from_params naming); None for batch-norm."""
+    """'z1_yu/W' -> ('Wy', 1) etc. (oracle/tf_shim.variables_from_params naming); None for batch-norm."""
     scope, var = name.rsplit("/", 1)
     if "/bn" in name:
         return None
@@ -70,16 +70,17 @@ def tf_name_to_param(name):
     return table[kind][0 if var == "W" else 1], i
 
 
-def model_grads(p, path, sizes, xr, Y, V, c):
+def model_grads(p, sizes, xr, Y, V, c):
     """gv_ of the reference's Model built on the shim with feeds (x, y, v, c) = the given rows: {tf name: grad}."""
-    from oracle.gen_golden_tfshim import _shim, extract
     n = p.n
     bnvars = [(np.ones(s), np.zeros(s), np.zeros(s), np.full(s, 1.0 - BN_EPS)) for s in p.hidden[:-1]]
-    feeds = {"x": (xr, False), "y": (Y, True), "trueY": (np.zeros((len(Y), n)), False), "v": (V, False), "c": (c, False)}
-    sh = _shim({"p": p, "bnvars": bnvars}, feeds)
-    ns = extract(path, ["Model"], {"tf": sh.tf, "tflearn": sh.tflearn, "np": np,
-                                   "variable_summaries": lambda *a, **k: None})
-    with contextlib.redirect_stdout(io.StringIO()):
+    sh = Shim(variables_from_params(p, bnvars))
+    for k, a, rg in (("x", xr, False), ("y", Y, True), ("trueY", np.zeros((len(Y), n)), False), ("v", V, False),
+                     ("c", c, False)):
+        sh.feed(k, a, requires_grad=rg)
+    ns = refcode.extract("multi-label-cls/icnn_ebundle.py", ["Model"],
+                         {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
+    with refcode.quiet():
         model = ns["Model"](p.m, n, list(sizes), None)
     assert not sh.unused_variables(), sh.unused_variables()
     assert model.szs == p.hidden
@@ -87,25 +88,22 @@ def model_grads(p, path, sizes, xr, Y, V, c):
 
 
 def generate():
-    from oracle import picnn_np
-    from oracle.gen_golden import _load, REF
-    from oracle.gen_golden_grad import extract as extract_fn, train_step_fd_golden
-    ref_pc = _load("ref_pc", os.path.join(REF, "lib/bundle_entropy.py"))
+    ref_pc = refcode.load("ref_pc", "lib/bundle_entropy.py")
     grad_fns = {"xent": ("multi-label-cls/icnn_ebundle.py", "crossEntrGrad", None),
                 "mse": ("completion/icnn_ebundle.py", "mseGrad", "n")}
-    ml = os.path.join(REF, "multi-label-cls/icnn_ebundle.py")
     out = {}
     for tag in CASES:
         p, x, y0, trueY, nIter, sizes = case_inputs(tag)
         B = len(x)
-        with contextlib.redirect_stdout(io.StringIO()), np.errstate(all="ignore"):
+        with refcode.quiet():
             yN, G, h, lam, ys, nIters = ref_pc.solveBatch(picnn_np.make_fg(p, x), y0.copy(), nIter=nIter)
         counts = np.array([len(g) for g in G])
         for loss in LOSSES:
-            path, fname, oshape = grad_fns[loss]
-            fn = extract_fn(os.path.join(REF, path), fname)
-            fd = train_step_fd_golden(os.path.join(REF, path), fname, fn, B, x, trueY, G, yN, ys, lam,
-                                      (p.n,) if oshape else None)
+            rel, fname, oshape = grad_fns[loss]
+            train_step_fd = refcode.extract(rel, [fname, "Model.train_step_fd"], {"np": np})["train_step_fd"]
+            stub = types.SimpleNamespace(x_="x", y_="y", v_="v", c_="c", outputSz=(p.n,) if oshape else None)
+            with np.errstate(all="ignore"):
+                fd = train_step_fd(stub, B, x, trueY, G, yN, ys, lam)
             assert np.array_equal(fd["x"], np.repeat(x, counts, axis=0))
             f32 = lambda a: np.asarray(a, dtype=np.float32).astype(np.float64)  # noqa: E731
             Y, V, c = f32(fd["y"]), f32(fd["v"]), f32(fd["c"])
@@ -115,7 +113,7 @@ def generate():
             per = {}
             for u in range(B):
                 s = slice(off[u], off[u + 1])
-                gv = model_grads(p, ml, sizes, np.repeat(x[u:u + 1], counts[u], axis=0), Y[s], V[s], c[s]) \
+                gv = model_grads(p, sizes, np.repeat(x[u:u + 1], counts[u], axis=0), Y[s], V[s], c[s]) \
                     if counts[u] else {}
                 for name, ga in gv.items():
                     per.setdefault(name, np.zeros((B,) + ga.shape))[u] = ga
@@ -130,13 +128,5 @@ def generate():
     return out
 
 
-def main():
-    out = generate()
-    # a subdirectory: tests/test_oracle_golden.py runs every tests/golden/*.npz as a solveBatch case
-    path = os.path.join(ROOT, "tests", "golden", "training", "bundle_grad.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, len(out), "arrays,", os.path.getsize(path) // 1024, "KB")
-
-
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_bundle_grad",))

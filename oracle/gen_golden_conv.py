@@ -9,18 +9,14 @@ cases have non-zero biases in every layer that has one and non-identity batch-no
 Weights and inputs are regenerated from seeds by ``case`` (shared with the tests); only outputs are stored.
 
 TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
-Usage:  python oracle/gen_golden_conv.py   -> tests/golden/conv/conv_picnn.npz
+Usage:  python -m oracle.gen_golden_conv   -> tests/golden/conv/conv_picnn.npz
 """
-import contextlib
-import io
-import os
-import sys
-
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from oracle import refcode, regen
+from oracle.tf_shim import Shim, tensor_get_shape
 
+GOLDEN = "conv/conv_picnn.npz"
 CASES = {"conv_bn_olivetti": (3, 64, 32, 11), "conv_bn_odd": (4, 17, 9, 12)}     # tag -> (B, H, W, seed)
 
 
@@ -31,8 +27,7 @@ def _f32(a):
 def case(tag):
     """-> (variables {name: float64 array, float32-representable}, x [B, H*W], y [B, H*W], H, W)."""
     import torch
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    from conv_picnn import ConvPICNN
+    from oracle.conv_picnn import ConvPICNN
     from oracle.gen_golden_tfshim import conv_variables
     B, H, W, seed = CASES[tag]
     v = conv_variables(ConvPICNN(H, W, seed=seed, dtype=torch.float64))
@@ -57,9 +52,7 @@ def case(tag):
     return v, x, y, H, W
 
 
-def run(tag, ref):
-    from oracle.gen_golden_tfshim import extract
-    from oracle.tf_shim import Shim, tensor_get_shape
+def run(tag):
     v, x, y, H, W = case(tag)
     B = x.shape[0]
     sh = Shim(v)
@@ -68,25 +61,21 @@ def run(tag, ref):
                      ("trueY", np.zeros((B, H, W, 1)), False), ("v", rs.randn(B, H * W), False), ("c", rs.randn(B), False),
                      ("l_yN", np.zeros(()), False), ("nBundleIter", np.zeros(B), False), ("nActive", np.zeros(B), False)):
         sh.feed(k, a, requires_grad=rg)
-    ns = extract(os.path.join(ref, "completion/icnn_ebundle.py"), ["Model"],
-                 {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
-    with contextlib.redirect_stdout(io.StringIO()), tensor_get_shape():
+    ns = refcode.extract("completion/icnn_ebundle.py", ["Model"],
+                         {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
+    with refcode.quiet(), tensor_get_shape():
         model = ns["Model"]([H, W, 1], [H, W, 1], None)
     assert not sh.unused_variables(), sh.unused_variables()
     return model.E_.detach().numpy(), model.dE_dyFlat_.detach().numpy()
 
 
-def main():
-    ref = os.environ.get("ICNN_REFERENCE_DIR", "")
+def generate():
     out = {}
     for tag in CASES:
-        out[tag + "_f"], out[tag + "_g"] = run(tag, ref)
+        out[tag + "_f"], out[tag + "_g"] = run(tag)
         print(tag, "f", out[tag + "_f"], "max|g|", np.abs(out[tag + "_g"]).max())
-    path = os.path.join(ROOT, "tests", "golden", "conv", "conv_picnn.npz")
-    os.makedirs(os.path.dirname(path), exist_ok=True)
-    np.savez_compressed(path, **out)
-    print("wrote", path, os.path.getsize(path) // 1024, "KB")
+    return out
 
 
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_conv",))

@@ -13,18 +13,14 @@ its projections on four fixed random vectors (gen_golden_conv_grad.probe, [B, 4]
 variable gv_ holds.
 
 TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
-Usage:  python oracle/gen_golden_conv_gd_grad.py   -> tests/golden/conv/conv_gd_grad.npz
+Usage:  python -m oracle.gen_golden_conv_gd_grad   -> tests/golden/conv/conv_gd_grad.npz
 """
-import contextlib
-import io
-import os
-import sys
-
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from oracle import refcode, regen
+from oracle.tf_shim import Shim, tensor_get_shape
 
+GOLDEN = "conv/conv_gd_grad.npz"
 CASES = ("conv_bn_odd", "conv_bn_olivetti")     # tags of oracle/gen_golden_conv.py
 N_GD_ITER = 30                                  # completion/icnn.back.py --nGdIter default
 MAX_WHOLE = 4096
@@ -41,18 +37,16 @@ def case_inputs(tag):
     return v, x, y0, trueY, H, W
 
 
-def model_outputs(v, path, H, W, x, y0, trueY, nGdIter):
+def model_outputs(v, H, W, x, y0, trueY, nGdIter):
     """(yn_, mse_, {name: gradient}) of the reference's back-optimisation Model built on the shim with these feeds."""
-    from oracle.gen_golden_tfshim import extract
-    from oracle.tf_shim import Shim, tensor_get_shape
     B = len(x)
     sh = Shim(v)
     for k, a, rg in (("x", x.reshape(B, H, W, 1), False), ("y", y0.reshape(B, H, W, 1), True),
                      ("trueY", trueY.reshape(B, H, W, 1), False)):
         sh.feed(k, a, requires_grad=rg)
-    ns = extract(path, ["Model"], {"tf": sh.tf, "tflearn": sh.tflearn, "np": np,
-                                   "variable_summaries": lambda *a, **k: None})
-    with contextlib.redirect_stdout(io.StringIO()), tensor_get_shape():
+    ns = refcode.extract("completion/icnn.back.py", ["Model"],
+                         {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
+    with refcode.quiet(), tensor_get_shape():
         model = ns["Model"]([H, W, 1], [H, W, 1], None, nGdIter)
     assert not sh.unused_variables(), sh.unused_variables()
     grads = {var.name[:-2]: g.detach().numpy().copy() for g, var in model.gv_}
@@ -61,10 +55,9 @@ def model_outputs(v, path, H, W, x, y0, trueY, nGdIter):
 
 def generate():
     import torch
-    from oracle.gen_golden import REF
     from oracle.gen_golden_conv_grad import probe
+    threads = torch.get_num_threads()
     torch.set_num_threads(1)          # the same float64 sums on every regeneration
-    path = os.path.join(REF, "completion/icnn.back.py")
     out = {}
     for tag in CASES:
         v, x, y0, trueY, H, W = case_inputs(tag)
@@ -72,7 +65,7 @@ def generate():
         per, names, yn, mse = {}, None, np.zeros((B, H * W)), np.zeros(B)
         for u in range(B):
             s = slice(u, u + 1)
-            yn[u], mse[u], gv = model_outputs(v, path, H, W, x[s], y0[s], trueY[s], N_GD_ITER)
+            yn[u], mse[u], gv = model_outputs(v, H, W, x[s], y0[s], trueY[s], N_GD_ITER)
             names = sorted(gv) if names is None else names
             assert sorted(gv) == names
             for name, ga in gv.items():
@@ -86,15 +79,9 @@ def generate():
         out[tag + "_yn"], out[tag + "_mse"] = yn, mse
         out[tag + "_nGdIter"] = np.array(N_GD_ITER)
         print(tag, "B", B, "gv_", len(names), "whole", sum(k.startswith(tag + "_grad_") for k in out), flush=True)
+    torch.set_num_threads(threads)    # the generators run after this one compute as they do alone
     return out
 
 
-def main():
-    out = generate()
-    path = os.path.join(ROOT, "tests", "golden", "conv", "conv_gd_grad.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, len(out), "arrays,", os.path.getsize(path) // 1024, "KB")
-
-
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_conv_gd_grad",))

@@ -1,16 +1,14 @@
 #!/usr/bin/env python
 """Golden vectors for d mse / d theta through the unrolled momentum-GD loop, from torch float64
 autograd on the restated training graph (oracle/gd_grad_torch.py; the reference's TF graph,
-multi-label-cls/icnn-back.py:116-139, cannot run here).  TEST INFRASTRUCTURE ONLY."""
-import os
-import sys
-
+multi-label-cls/icnn-back.py:116-139, cannot run here).  TEST INFRASTRUCTURE ONLY.
+Usage:  python -m oracle.gen_golden_gd_grad   -> tests/golden/gd_grad.npz"""
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from oracle import synth  # noqa: E402
-from oracle.gd_grad_torch import torch_unrolled_grads  # noqa: E402
+from oracle import regen, synth
+from oracle.gd_grad_torch import torch_unrolled_grads
+
+GOLDEN = "gd_grad.npz"
 
 CASES = {
     # tag: (config, B, nIter, lr, momentum)   -- icnn-back.py defaults are lr .01, momentum .3, 30 its
@@ -23,7 +21,7 @@ def true_labels(B, n, seed=11):
     return (np.random.RandomState(seed).uniform(size=(B, n)) < 0.3).astype(np.float64)
 
 
-def main():
+def generate():
     out = {}
     for tag, (name, B, nIter, lr, mom) in CASES.items():
         p, x, y0 = synth.make_inputs(name, B=B)
@@ -36,10 +34,8 @@ def main():
             for i, g in enumerate(G[k]):
                 if g is not None:
                     out["%s_%s%d" % (tag, k, i)] = g
-    path = os.path.join(ROOT, "tests", "golden", "gd_grad.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, len(out), "arrays", os.path.getsize(path), "bytes")
+    return out
 
 
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_gd_grad",))

@@ -10,7 +10,7 @@ Executed reference code (paths relative to a locuslab/icnn checkout):
   RL/src/icnn.py                   class Agent: negQ (:325-404), bundle_entropy (:148-158); entropy (:455-458)
   RL/src/bundle_entropy.py         solveBatch (imported unchanged, called BY Agent.bundle_entropy)
   completion/icnn_ebundle.py       class Model: __init__ (:105-161) and f (:337-452): the CONVOLUTIONAL PICNN of the
-                                   Olivetti experiment -> E_, dE_dy_; pins tests/conv_picnn.py, the user-side ``fg`` the
+                                   Olivetti experiment -> E_, dE_dy_; pins oracle/conv_picnn.py, the user-side ``fg`` the
                                    GPU callback-mode test drives K2 with
 
 The goldens pin oracle/picnn_np.py (f, df/dy, gates incl. batch-norm, momentum GD, the RL affine wrapper) and
@@ -19,22 +19,17 @@ compared with the device kernels in tests/test_gpu_picnn.py.  Weights and inputs
 ``case_inputs`` (shared with the tests); only outputs are stored.
 
 TEST INFRASTRUCTURE ONLY; needs a checkout of the reference at $ICNN_REFERENCE_DIR.
-Usage:  python oracle/gen_golden_tfshim.py
+Usage:  python -m oracle.gen_golden_tfshim   -> tests/golden/picnn_tfshim.npz
 """
-import ast
-import contextlib
-import io
-import os
-import sys
 import types
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from icnn_b200 import workloads  # noqa: E402  (pure-numpy input generator)
+from icnn_b200 import workloads  # (pure-numpy input generator)
+from oracle import refcode, regen
+from oracle.tf_shim import Shim, tensor_get_shape, variables_from_params
 
-REF = os.environ.get("ICNN_REFERENCE_DIR", "")
+GOLDEN = "picnn_tfshim.npz"
 BN_EPS = 1e-5
 
 
@@ -123,56 +118,23 @@ CASES = ["ml_fg_c3", "ml_fg_bn", "rl_fg_c4", "rl_fg_entr_c4", "rl_act_c4", "trac
 # reference code on the shim
 # --------------------------------------------------------------------------------------------------------
 
-def variables_from_params(p, bnvars=None, prefix=""):
-    """PicnnParams -> {tensorflow variable name: array}, the naming of the reference's variable scopes
-    (multi-label-cls/icnn_ebundle.py:341,353,356,363,366,372; RL/src/icnn.py:346,361,366,373,377,384)."""
-    v = {}
-    for i in range(p.L):
-        v["%su%d/W" % (prefix, i)] = p.Wu[i]
-        v["%su%d/b" % (prefix, i)] = p.bu[i]
-        if bnvars is not None and i < p.L - 1:
-            for nm, a in zip(("gamma", "beta", "moving_mean", "moving_variance"), bnvars[i]):
-                v["%su%d/bn/%s" % (prefix, i, nm)] = a
-    for i in range(p.L + 1):
-        if i > 0:
-            v["%sz%d_zu_u/W" % (prefix, i)] = p.Wzu[i]
-            v["%sz%d_zu_u/b" % (prefix, i)] = p.bzu[i]
-            v["%sz%d_zu_proj/W" % (prefix, i)] = p.Wz[i]
-        v["%sz%d_yu_u/W" % (prefix, i)] = p.Wyu[i]
-        v["%sz%d_yu_u/b" % (prefix, i)] = p.byu[i]
-        v["%sz%d_yu/W" % (prefix, i)] = p.Wy[i]
-        v["%sz%d_u/W" % (prefix, i)] = p.Wzx[i]
-        v["%sz%d_u/b" % (prefix, i)] = p.bzx[i]
-    return v
-
-
-def extract(path, names, namespace):
-    """exec the top-level class / function definitions ``names`` of a reference file, verbatim, in ``namespace``."""
-    tree = ast.parse(open(path).read())
-    body = [n for n in tree.body if isinstance(n, (ast.ClassDef, ast.FunctionDef)) and n.name in names]
-    assert len(body) == len(names), (path, names)
-    exec(compile(ast.Module(body=body, type_ignores=[]), path, "exec"), namespace)
-    return namespace
-
-
 def _shim(c, feeds, prefix=""):
-    from oracle.tf_shim import Shim
     sh = Shim(variables_from_params(c["p"], c.get("bnvars"), prefix))
     for k, (a, rg) in feeds.items():
         sh.feed(k, a, requires_grad=rg)
     return sh
 
 
-def run_multilabel_model(c, path, ctor_args):
+def run_multilabel_model(c, rel, ctor_args):
     """Model(...) of a multi-label script: building it evaluates the whole graph on the fed tensors."""
     B, n = c["y"].shape
     rs = np.random.RandomState(5)
     feeds = {"x": (c["x"], False), "y": (c["y"], True), "trueY": (c.get("trueY", np.zeros((B, n))), False),
              "v": (rs.randn(B, n), False), "c": (rs.randn(B), False)}
     sh = _shim(c, feeds)
-    ns = extract(path, ["Model"], {"tf": sh.tf, "tflearn": sh.tflearn, "np": np,
-                                   "variable_summaries": lambda *a, **k: None})
-    with contextlib.redirect_stdout(io.StringIO()):
+    ns = refcode.extract(rel, ["Model"], {"tf": sh.tf, "tflearn": sh.tflearn, "np": np,
+                                          "variable_summaries": lambda *a, **k: None})
+    with refcode.quiet():
         model = ns["Model"](c["p"].m, c["p"].n, *ctor_args, None)
     assert not sh.unused_variables(), sh.unused_variables()
     assert model.szs == c["p"].hidden
@@ -203,10 +165,9 @@ CONV_CASES = {"conv_small": (4, 16, 8, 3), "conv_olivetti": (2, 64, 32, 1)}     
 
 
 def conv_case(tag):
-    """-> (ConvPICNN float64, x [B, H*W], y [B, H*W]) of tests/conv_picnn.py, seeded."""
+    """-> (ConvPICNN float64, x [B, H*W], y [B, H*W]) of oracle/conv_picnn.py, seeded."""
     import torch
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    from conv_picnn import ConvPICNN
+    from oracle.conv_picnn import ConvPICNN
     B, H, W, seed = CONV_CASES[tag]
     net = ConvPICNN(H, W, seed=seed, dtype=torch.float64)
     rs = np.random.RandomState(100 + seed)
@@ -214,19 +175,24 @@ def conv_case(tag):
 
 
 def conv_variables(net):
-    """tests/conv_picnn.py parameters -> the reference's variable names and TensorFlow layouts: conv kernels
-    [k, k, c_in, c_out]; the dense layers behind the last conv see its feature map flattened in NHWC order."""
-    from conv_picnn import CONVS, FCS
+    """oracle/conv_picnn.py parameters -> the reference's variable names and TensorFlow layouts: conv kernels
+    [k, k, c_in, c_out]; the dense layers behind the last conv see its feature map flattened in NHWC order.  The
+    architecture is read off the parameters, not off a module's CONVS / FCS, so any net of that class converts: each
+    conv layer's stride is the reference's for its kernel size (8 -> 4, 4 -> 2, 3 -> 1), checked against the width
+    of the first dense layer."""
     P = net.P
     v = {}
-    nc = len(CONVS)
+    nc = sum(k.startswith("y_red") for k in P)
     cw = lambda w: w.permute(2, 3, 1, 0).numpy()                                    # noqa: E731
     h, w = net.H, net.W
-    for (_nf, _k, s_) in CONVS:
+    for i in range(nc):
+        k = P["u%d" % i][0].shape[-1]
+        s_ = k // 2 if k % 2 == 0 else 1
         h, w = -(-h // s_), -(-w // s_)
-    C = CONVS[-1][0]
+    C = P["u%d" % (nc - 1)][0].shape[0]
+    assert P["u%d" % nc][0].shape[0] == C * h * w, "the conv strides do not follow the kernel-size rule"
     perm = np.arange(C * h * w).reshape(C, h, w).transpose(1, 2, 0).reshape(-1)     # NHWC position -> NCHW index
-    for i in range(nc + len(FCS)):
+    for i in range(sum(k.startswith("z_u") for k in P)):
         conv = i < nc
         Wu, bu = P["u%d" % i]
         v["u%d/W" % i] = cw(Wu) if conv else (Wu.numpy()[perm] if i == nc else Wu.numpy())
@@ -258,7 +224,6 @@ def conv_variables(net):
 
 
 def run_completion_model(tag):
-    from oracle.tf_shim import Shim, tensor_get_shape
     net, x, y = conv_case(tag)
     B, H, W, _ = CONV_CASES[tag]
     sh = Shim(conv_variables(net))
@@ -267,9 +232,9 @@ def run_completion_model(tag):
                      ("trueY", np.zeros((B, H, W, 1)), False), ("v", rs.randn(B, H * W), False), ("c", rs.randn(B), False),
                      ("l_yN", np.zeros(()), False), ("nBundleIter", np.zeros(B), False), ("nActive", np.zeros(B), False)):
         sh.feed(k, a, requires_grad=rg)
-    ns = extract(os.path.join(REF, "completion/icnn_ebundle.py"), ["Model"],
-                 {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
-    with contextlib.redirect_stdout(io.StringIO()), tensor_get_shape():
+    ns = refcode.extract("completion/icnn_ebundle.py", ["Model"],
+                         {"tf": sh.tf, "tflearn": sh.tflearn, "np": np, "variable_summaries": lambda *a, **k: None})
+    with refcode.quiet(), tensor_get_shape():
         model = ns["Model"]([H, W, 1], [H, W, 1], None)
     assert not sh.unused_variables(), sh.unused_variables()
     return model.E_.detach().numpy(), model.dE_dyFlat_.detach().numpy(), len(sh.created)
@@ -277,14 +242,12 @@ def run_completion_model(tag):
 
 def generate():
     """-> {name: array}: every golden of tests/golden/picnn_tfshim.npz, recomputed from the reference checkout."""
-    sys.path.insert(0, os.path.join(REF, "RL", "src"))
-    from oracle.gen_golden import _load
     out = {}
 
     # ---- multi-label Model (bundle-entropy script): E_ and dE_dy_ ------------------------------------------------
     for tag in ("ml_fg_c3", "ml_fg_bn"):
         c = case_inputs(tag)
-        sh, model = run_multilabel_model(c, os.path.join(REF, "multi-label-cls/icnn_ebundle.py"), (list(c["layerSizes"]),))
+        sh, model = run_multilabel_model(c, "multi-label-cls/icnn_ebundle.py", (list(c["layerSizes"]),))
         out[tag + "_f"] = model.E_.detach().numpy()
         out[tag + "_g"] = model.dE_dy_.detach().numpy()
         out[tag + "_g_entr"] = model.dE_entr_dy_.detach().numpy()
@@ -292,9 +255,9 @@ def generate():
 
     # ---- RL Agent.negQ and Agent.bundle_entropy ---------------------------------------------------------------
     flags = types.SimpleNamespace(l1size=200, l2size=200, icnn_bn=False, lrelu=0.01)
-    ref_rl = _load("bundle_entropy", os.path.join(REF, "RL/src/bundle_entropy.py"))
+    ref_rl = refcode.load("bundle_entropy", "RL/src/bundle_entropy.py")
     agent_ns = {"np": np, "FLAGS": flags, "bundle_entropy": ref_rl, "variable_summaries": lambda *a, **k: None}
-    extract(os.path.join(REF, "RL/src/icnn.py"), ["Agent", "entropy"], agent_ns)
+    refcode.extract("RL/src/icnn.py", ["Agent", "entropy"], agent_ns)
     c = case_inputs("rl_fg_c4")
     # the wrapper of Agent.bundle_entropy (:150-153), applied by hand for the fg golden: a = 2x - 1, grad *= 2
     _agent, f, g = run_negq(c, agent_ns, c["x"], 2.0 * c["y"] - 1.0)
@@ -307,26 +270,26 @@ def generate():
     def func(obs, act):                      # what Fun([obs, act], [negQ, act_grad]) returns (:107)
         _a, f_, g_ = run_negq(c, agent_ns, obs, act)
         return f_, g_
-    with contextlib.redirect_stdout(io.StringIO()), np.errstate(all="ignore"):
+    with refcode.quiet():
         out["rl_act_c4_act"] = agent.bundle_entropy(func, c["x"])
     print("rl_act_c4 act[0]", out["rl_act_c4_act"][0])
 
     # ---- the reference's own benchmark of the inner loop (multi-label-cls/ebundle-vs-gd.py:84-107): its Model graph as fg,
     # its lib/bundle_entropy.solveBatch, its entr(), and the callback (t, es, x) -> mean(es - entr(x)) it plots
     c = case_inputs("trace_c3")
-    ref_pc = _load("ref_pc_trace", os.path.join(REF, "lib/bundle_entropy.py"))
-    entr = extract(os.path.join(REF, "multi-label-cls/ebundle-vs-gd.py"), ["entr"], {"np": np})["entr"]
+    ref_pc = refcode.load("ref_pc_trace", "lib/bundle_entropy.py")
+    entr = refcode.extract("multi-label-cls/ebundle-vs-gd.py", ["entr"], {"np": np})["entr"]
     trace, iters = [], []
 
     def fg_ref(yhats):                       # sess.run([model.E_, model.dE_dy_]) (:88-91)
         cc = dict(c, y=np.asarray(yhats, dtype=np.float64))
-        _sh, model = run_multilabel_model(cc, os.path.join(REF, "multi-label-cls/icnn_ebundle.py"), (list(c["layerSizes"]),))
+        _sh, model = run_multilabel_model(cc, "multi-label-cls/icnn_ebundle.py", (list(c["layerSizes"]),))
         return model.E_.detach().numpy().copy(), model.dE_dy_.detach().numpy().copy()
 
     def cb(iterNum, es, x):                  # :93-98
         iters.append(iterNum)
         trace.append(np.mean(es - entr(x)))
-    with contextlib.redirect_stdout(io.StringIO()), np.errstate(all="ignore"):
+    with refcode.quiet():
         r = ref_pc.solveBatch(fg_ref, c["y"].copy(), nIter=c["nIter"], callback=cb)
     out["trace_c3_iters"], out["trace_c3_f_minus_H"], out["trace_c3_yN"] = np.array(iters), np.array(trace), r[0]
     print("trace_c3 mean(f - H) per iteration:", np.round(trace, 3))
@@ -336,7 +299,7 @@ def generate():
         c = case_inputs(tag)
         args = types.SimpleNamespace(layerSizes=list(c["layerSizes"]), inference_lr=c["lr"],
                                      inference_momentum=c["momentum"], inference_nIter=c["nIter"])
-        sh, model = run_multilabel_model(c, os.path.join(REF, "multi-label-cls/icnn-back.py"), (args,))
+        sh, model = run_multilabel_model(c, "multi-label-cls/icnn-back.py", (args,))
         out[tag + "_yN"] = model.yn_.detach().numpy()
         out[tag + "_energies"] = model.energies_.detach().numpy()
         out[tag + "_mse"] = np.array(float(model.mse_.detach()))
@@ -359,12 +322,5 @@ def generate():
     return out
 
 
-def main():
-    out = generate()
-    path = os.path.join(ROOT, "tests", "golden", "picnn_tfshim.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, len(out), "arrays,", os.path.getsize(path) // 1024, "KB")
-
-
 if __name__ == "__main__":
-    main()
+    regen.main(("gen_golden_tfshim",))

@@ -269,3 +269,26 @@ class Shim:
             leaky_relu=lambda x, alpha=0.1: torch.relu(_t(x)) - alpha * torch.relu(-_t(x)))
         tl.is_training = lambda flag: None
         return tl
+
+
+def variables_from_params(p, bnvars=None, prefix=""):
+    """PicnnParams -> {tensorflow variable name: array}, the naming of the reference's variable scopes
+    (multi-label-cls/icnn_ebundle.py:341,353,356,363,366,372; RL/src/icnn.py:346,361,366,373,377,384)."""
+    v = {}
+    for i in range(p.L):
+        v["%su%d/W" % (prefix, i)] = p.Wu[i]
+        v["%su%d/b" % (prefix, i)] = p.bu[i]
+        if bnvars is not None and i < p.L - 1:
+            for nm, a in zip(("gamma", "beta", "moving_mean", "moving_variance"), bnvars[i]):
+                v["%su%d/bn/%s" % (prefix, i, nm)] = a
+    for i in range(p.L + 1):
+        if i > 0:
+            v["%sz%d_zu_u/W" % (prefix, i)] = p.Wzu[i]
+            v["%sz%d_zu_u/b" % (prefix, i)] = p.bzu[i]
+            v["%sz%d_zu_proj/W" % (prefix, i)] = p.Wz[i]
+        v["%sz%d_yu_u/W" % (prefix, i)] = p.Wyu[i]
+        v["%sz%d_yu_u/b" % (prefix, i)] = p.byu[i]
+        v["%sz%d_yu/W" % (prefix, i)] = p.Wy[i]
+        v["%sz%d_u/W" % (prefix, i)] = p.Wzx[i]
+        v["%sz%d_u/b" % (prefix, i)] = p.bzx[i]
+    return v

@@ -4,14 +4,12 @@ reference graph's goldens; the descriptor struct matches the C header."""
 import ctypes as C
 import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def _olivetti_vars():
@@ -57,10 +55,10 @@ def test_parse_variables_checks_the_strides_against_the_dense_width():
 
 
 def test_torch_helper_from_the_variables_matches_the_reference_goldens():
-    """tests/conv_energy.py (float64, literal batch-norm, NHWC flattening) against E_ / dE_dy_ of the reference's
+    """oracle/conv_energy.py (float64, literal batch-norm, NHWC flattening) against E_ / dE_dy_ of the reference's
     own completion Model with non-zero biases and non-identity batch-norm statistics (17 x 9 included)."""
-    import conv_energy
     from icnn_b200.conv_picnn import parse_variables
+    from oracle import conv_energy
     from oracle.gen_golden_conv import CASES, case
     gold = np.load(os.path.join(ROOT, "tests", "golden", "conv", "conv_picnn.npz"))
     for tag in CASES:

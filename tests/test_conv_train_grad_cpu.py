@@ -1,6 +1,6 @@
 """CPU checks of the conv-PICNN training gradient: the C ABI struct matches the header and null arguments are refused
 before any device is touched; the float64 oracle (oracle/conv_train_grad_torch.py) evaluates the energy of
-tests/conv_energy.py (pinned to the reference's graph) and its gradient agrees with central finite differences."""
+oracle/conv_energy.py (pinned to the reference's graph) and its gradient agrees with central finite differences."""
 import ctypes as C
 import os
 import re
@@ -49,9 +49,7 @@ def _tiny(seed=1):
 
 
 def test_oracle_energy_is_the_reference_energy():
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import conv_energy
+    from oracle import conv_energy
     spec, x, Y, _V, _c, counts = _tiny()
     iu = np.repeat(np.arange(len(counts)), counts)
     V64 = {k: torch.as_tensor(a, dtype=torch.float64) for k, a in spec.vars.items()}

@@ -1,6 +1,6 @@
 """The float64 conv training-gradient oracle (oracle/conv_train_grad_torch.py) against the reference's own training
 step (tests/golden/conv/conv_train_grad.npz: solveBatch, mseGrad, Model.train_step_fd and Model.__init__'s gv_ on the
-TF shim), and the regeneration of that golden from a reference checkout (skipped without one)."""
+TF shim)."""
 import os
 import types
 
@@ -54,14 +54,3 @@ def test_oracle_reproduces_the_reference_training_step(tag):
             err = np.abs(got - ref).max()
             assert err <= 1e-9 * max(1.0, np.abs(ref).max()), (u, name, err)
 
-
-def test_golden_regenerates_from_the_reference():
-    ref = os.environ.get("ICNN_REFERENCE_DIR", "")
-    if not ref or not os.path.isfile(os.path.join(ref, "completion", "icnn_ebundle.py")):
-        pytest.skip("no reference checkout at $ICNN_REFERENCE_DIR")
-    from oracle.gen_golden_conv_grad import generate
-    gold = np.load(GOLDEN)
-    out = generate()
-    assert set(out) == set(gold.files)
-    for k, a in out.items():
-        np.testing.assert_array_equal(np.asarray(a, dtype=gold[k].dtype), gold[k], err_msg=k)

@@ -628,7 +628,7 @@ def test_callback_mode_with_a_conv_picnn_fg():
     default TF32 convolutions the user's g carries 1e-3 relative noise and half the samples move by
     2e-2 -- a property of that fg, which is why TF32 is switched off here)."""
     import torch
-    from conv_picnn import ConvPICNN
+    from oracle.conv_picnn import ConvPICNN
     from icnn_b200 import bundle_entropy as be
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False

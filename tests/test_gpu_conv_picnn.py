@@ -4,7 +4,6 @@ against callback mode and the float64 oracle, momentum GD, determinism and the s
 
 Accuracy criterion for f and g: max |device - float64| <= max(4 x the same error of the network evaluated in torch
 float32 with TF32 off, 1e-6 x max |float64|)."""
-import sys
 import os
 import warnings
 
@@ -12,16 +11,13 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import bundle_np
+from oracle import bundle_np, conv_energy
+from oracle import conv_picnn as helper
 
 pytestmark = pytest.mark.gpu
 np.seterr(all="ignore")
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-if HERE not in sys.path:
-    sys.path.insert(0, HERE)
-import conv_energy  # noqa: E402
-import conv_picnn as helper  # noqa: E402
 
 PINS = [(-1, -1), (0, 1), (1, 1), (2, 1), (1, 2), (1, 4), (1, 8)]     # (cfg, splitk) of icnn_tc_set_tuning
 

@@ -1,5 +1,5 @@
 """The RL agent's TD training gradient on the GPU (icnn_td_grad, icnn_b200.td_grad) against the reference's own code
-on the TF shim (tests/golden/rl/td_grad.npz) and the float64 oracle (tests/td_grad_np.py).
+on the TF shim (tests/golden/rl/td_grad.npz) and the float64 oracle (oracle/td_grad_np.py).
 
 Tolerance (test_gpu_bundle_grad's rule): every array must agree to RTOL = 2e-4 of its largest entry.  A float32
 evaluation of a row whose pre-activation sits within 1e-5 (relative) of zero can land on the other side of the leaky
@@ -14,8 +14,8 @@ import numpy as np
 import pytest
 import torch
 
-import td_grad_np as tg
 from oracle import bundle_grad_np as bg
+from oracle import td_grad_np as tg
 from oracle.gen_golden_bundle_grad import tf_name_to_param
 
 pytestmark = pytest.mark.gpu

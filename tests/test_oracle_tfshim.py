@@ -148,7 +148,7 @@ def test_unrolled_gd_and_training_gradient_match_the_reference_graph(tag, gold):
 
 @pytest.mark.parametrize("tag", ["conv_small", "conv_olivetti"])
 def test_conv_picnn_helper_matches_the_reference_graph(tag, gold):
-    """tests/conv_picnn.py -- the user-side ``fg`` the GPU callback-mode test drives K2 with at the Olivetti dims
+    """oracle/conv_picnn.py -- the user-side ``fg`` the GPU callback-mode test drives K2 with at the Olivetti dims
     (SURVEY.md 8d config 2) -- against E_ / dE_dy_ of the reference's own convolutional Model.__init__ / Model.f
     (completion/icnn_ebundle.py:105-161,337-452) executed on oracle/tf_shim.py: same wiring (u-path convs 32x8/4,
     64x4/2, 64x3/1 + FC 512, 1; y_red path; gates), 'SAME' padding, NHWC flatten order of the dense layers."""

@@ -1,11 +1,11 @@
 """CPU checks of the RL TD training gradient: the C ABI entries and their refusals before any device is touched, the
-Python argument errors, and properties of the float64 oracle (tests/td_grad_np.py)."""
+Python argument errors, and properties of the float64 oracle (oracle/td_grad_np.py)."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import td_grad_np as tg
+from oracle import td_grad_np as tg
 
 
 def test_abi_entries():

@@ -1,11 +1,11 @@
-"""The float64 oracle of the RL TD training step (tests/td_grad_np.py) against the reference's own Agent graph executed
-on the TF shim (tests/golden/rl/td_grad.npz, written by tools/gen_golden_td_grad.py)."""
+"""The float64 oracle of the RL TD training step (oracle/td_grad_np.py) against the reference's own Agent graph executed
+on the TF shim (tests/golden/rl/td_grad.npz, written by oracle/gen_golden_td_grad.py)."""
 import os
 
 import numpy as np
 import pytest
 
-import td_grad_np as tg
+from oracle import td_grad_np as tg
 from oracle.gen_golden_bundle_grad import tf_name_to_param
 
 

@@ -1,8 +1,8 @@
-"""The RL primitives of tests/tf_shim_rl.py against torch, the way test_tf_shim_cpu.py checks the shim's others."""
+"""The RL primitives of oracle/tf_shim_rl.py against torch, the way test_tf_shim_cpu.py checks the shim's others."""
 import numpy as np
 import torch
 
-from tf_shim_rl import RLShim
+from oracle.tf_shim_rl import RLShim
 
 
 def _shim():

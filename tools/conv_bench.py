@@ -3,7 +3,7 @@
 helper fg (TF32 off), which is how this energy ran before the fused path existed.
 
 Workloads ("C2-conv"): the reference's completion architecture ((32,8,4), (64,4,2), (64,3,1) / (512, 1)) at 64 x 32,
-lib PC solver, 30 iterations, B = 400 and the reference's trainBatchSz B = 70.  Weights: tests/conv_picnn.ConvPICNN(64,
+lib PC solver, 30 iterations, B = 400 and the reference's trainBatchSz B = 70.  Weights: oracle/conv_picnn.ConvPICNN(64,
 32, seed=2) via conv_variables; x ~ U(0, 1); y0 one fixed per-pixel vector from U(0.2, 0.8) for every sample.
 
 Prints one JSON line per (run, workload, arm) and a header line with the card, its power limit and SM clock, read in
@@ -24,7 +24,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 TF32_DENSE_TFLOPS = 495.0     # H100 SXM data sheet, dense TF32; 3xTF32 issues three MMAs per product
 
@@ -73,7 +72,7 @@ def main():
     args = ap.parse_args()
     import icnn_b200
     from icnn_b200 import bundle_entropy as be
-    from conv_picnn import ConvPICNN as Helper
+    from oracle.conv_picnn import ConvPICNN as Helper
     from oracle.gen_golden_tfshim import conv_variables
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False

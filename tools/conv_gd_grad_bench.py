@@ -1,5 +1,5 @@
 """Conv-PICNN GD training gradient at C2-conv: the reference's completion architecture ((32,8,4), (64,4,2), (64,3,1) /
-(512, 1)) at 64 x 32 with the weights of tools/conv_bench.py (tests/conv_picnn.ConvPICNN(64, 32, seed=2)), the back-
+(512, 1)) at 64 x 32 with the weights of tools/conv_bench.py (oracle/conv_picnn.ConvPICNN(64, 32, seed=2)), the back-
 optimisation mode's nIter = 30, lr = 0.01, momentum = 0.9, loss_scale = 2 255^2 / (B n), B = 70 (the reference's
 trainBatchSz) and 400.
 
@@ -24,7 +24,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 
@@ -40,7 +39,7 @@ def main():
     from icnn_b200.conv_picnn import _train_grad_buffers, parse_variables
     from icnn_b200.gd_grad import gd_grad
     from conv_bench import card, events_ms
-    from conv_picnn import ConvPICNN as Helper
+    from oracle.conv_picnn import ConvPICNN as Helper
     from oracle import conv_train_grad_torch as O
     from oracle.gen_golden_tfshim import conv_variables
     torch.backends.cudnn.allow_tf32 = False

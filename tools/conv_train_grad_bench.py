@@ -1,5 +1,5 @@
 """Conv-PICNN training gradient at C2-conv: the reference's completion architecture ((32,8,4), (64,4,2), (64,3,1) /
-(512, 1)) at 64 x 32 with the weights of tools/conv_bench.py (tests/conv_picnn.ConvPICNN(64, 32, seed=2)), 30 solver
+(512, 1)) at 64 x 32 with the weights of tools/conv_bench.py (oracle/conv_picnn.ConvPICNN(64, 32, seed=2)), 30 solver
 iterations, B = 70 (the reference's trainBatchSz) and 400.
 
 Per batch it prints R (the train_step_fd rows the solve leaves) and CUDA-event times of
@@ -22,7 +22,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 
@@ -37,7 +36,7 @@ def main():
     from icnn_b200.bundle_grad import _conv_launch, bundle_grad
     from icnn_b200.conv_picnn import parse_variables
     from conv_bench import card, events_ms
-    from conv_picnn import ConvPICNN as Helper
+    from oracle.conv_picnn import ConvPICNN as Helper
     from oracle import conv_train_grad_torch as O
     from oracle.gen_golden_tfshim import conv_variables
     torch.backends.cudnn.allow_tf32 = False

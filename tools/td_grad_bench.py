@@ -25,12 +25,11 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 import icnn_b200  # noqa: E402
 from icnn_b200 import adam  # noqa: E402
 from icnn_b200.bundle_grad import _launch as tg_launch, _prepare  # noqa: E402
 from icnn_b200.td_grad import _launch as td_launch, td_grad  # noqa: E402
-import td_grad_np as tgn  # noqa: E402
+from oracle import td_grad_np as tgn  # noqa: E402
 
 
 def gpu_info():
